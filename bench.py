@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- hot-path benchmark (contract in the task statement, tier section (4)).
+"""bench.py -- hot-path benchmark.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload c2|c3|c4]
-                    [--rows R]
+                    [--rows R] [--dump-outputs DIR]
 
 A "step" is one pass of convert_from_rows over the whole synthetic workload.
   value      : rows/s with the JCUDF row buffer already resident in HBM (CUDA events, max over ranks)
@@ -13,6 +13,8 @@ A "step" is one pass of convert_from_rows over the whole synthetic workload.
                InternalRow->ColumnarBatch, BASELINE.md section 3) on a bounded sample, host cores
 --impl reference times that CPU path alone (no JVM / libcudf in this image: the reference itself
 cannot run, SURVEY.md 8c).
+--dump-outputs DIR writes what the timed path computed in its last step as DIR/<name>.npy (float32 / float64, a
+fixed seeded row sample plus whole-output checksums, <= 64 MB), so that two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -47,13 +49,14 @@ def cycle(types, n):
     return [types[i % len(types)] for i in range(n)]
 
 WORKLOADS = {
-    # BASELINE.json configs[1]: 100M rows x 32 fixed-width cols convert_from_rows, 1xB200
+    # BASELINE.json configs[1]: 100M rows x 32 fixed-width cols convert_from_rows, 1xH100
     "c2": dict(name="C2: 100M rows x 32 fixed-width cols ([INT8,INT16,INT32,INT64,FLOAT32,FLOAT64,BOOL8,TIMESTAMP_US]x4) "
                     "convert_from_rows, 200 B rows, 20% nulls",
                types=[INT8, INT16, INT32, INT64, FLOAT32, FLOAT64, BOOL8, TS_US] * 4, rows=100_000_000, null_frac=0.2),
     # BASELINE.json configs[3]: store_sales, from_rows fused with xxhash64(ss_item_sk, ss_ticket_number)
+    # 200M rows: rows + source + output columns + hashes take ~62 GB of the H100's 80 GB
     "c4": dict(name="C4: TPC-DS store_sales (23 cols, 104 B rows) convert_from_rows + xxhash64 partition key in one call",
-               types=[INT32] * 9 + [INT64, INT32] + [DEC32] * 12, rows=400_000_000, null_frac=0.04, hash_keys=[1, 9]),
+               types=[INT32] * 9 + [INT64, INT32] + [DEC32] * 12, rows=200_000_000, null_frac=0.04, hash_keys=[1, 9]),
     # BASELINE.json configs[2]: 100M rows x 256 mixed cols (int32/int64/decimal128/utf8, 20% null), to+from rows.
     # ~390 GB of rows cannot be resident: a step streams 100M rows as `batches` x `batch_rows` conversions over a
     # resident pool of distinct <=2 GiB batches (each batch is what one LIST<INT8> column / one JNI call carries).
@@ -95,7 +98,7 @@ def load_peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s)"
 
 
 def gpu_local_cpus(torch, index: int):
@@ -145,7 +148,7 @@ class NumaBind:
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     def __init__(self, index: int):
         self.index = index
@@ -207,6 +210,109 @@ def box_copy_gbs(torch):
 def algorithmic_bytes_per_row(types, row_size, hashed=False):
     """SURVEY 8(d): read the padded row + write every column element + ncols/8 mask bytes (+ 8 B hash)."""
     return row_size + sum(SIZE[t] for t in types) + len(types) / 8.0 + (8 if hashed else 0)
+
+
+# ---------------------------------------------------------------------------------------------------
+# --dump-outputs: what the timed path computed in its last step.  The outputs are many GB, so every array is a
+# fixed, seeded row sample (the same rows for every run with the same arguments) in a float type that holds the
+# values exactly, plus exact whole-output checksums (byte sums, valid counts) that catch a difference anywhere.
+DUMP_SAMPLE_ROWS = 2048
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def sample_rows(n, seed=20260101):
+    return np.sort(np.random.default_rng(seed).integers(0, n, min(n, DUMP_SAMPLE_ROWS))) if n > 0 else np.zeros(0, np.int64)
+
+
+def exact_f64(b):
+    """uint8 [k, w] element bytes -> float64 holding them exactly: int8 / int16 values for w < 4, int32 words otherwise."""
+    b = np.ascontiguousarray(b)
+    if b.shape[1] < 4:
+        return b.view(np.int8 if b.shape[1] == 1 else np.int16)[:, 0].astype(np.float64)
+    v = b.view(np.int32).astype(np.float64)
+    return v[:, 0] if b.shape[1] == 4 else v
+
+
+def as_bytes(torch, t):
+    return t.reshape(-1).view(torch.uint8) if t is not None else None
+
+
+def gather_elems(torch, data, idx, w):
+    """bytes [k, w] of the w-byte elements at rows idx (device tensor)."""
+    pos = (idx.unsqueeze(1) * w + torch.arange(w, device=idx.device)).reshape(-1)
+    return as_bytes(torch, data)[pos].view(-1, w).cpu().numpy()
+
+
+def gather_lists(torch, offsets, data, idx):
+    """lengths (float64 [k]) and bytes (float32 [k, longest], -1 past a list's end) of the lists idx of offsets/data."""
+    o = offsets.reshape(-1)
+    start, end = o[idx].long(), o[idx + 1].long()
+    lens = end - start
+    width = int(lens.max()) if lens.numel() else 0
+    j = torch.arange(width, device=idx.device)
+    ok = j < lens.unsqueeze(1)
+    d = as_bytes(torch, data)
+    if d is not None and d.numel():
+        vals = d[torch.where(ok, start.unsqueeze(1) + j, 0)].float()
+    else:
+        vals = torch.zeros(ok.shape, device=idx.device)
+    return lens.double().cpu().numpy(), torch.where(ok, vals, -1.0).cpu().numpy().astype(np.float32)
+
+
+def byte_sum(torch, t):
+    b = as_bytes(torch, t)
+    if b is None:
+        return 0.0
+    return float(sum(int(b[o:o + (1 << 26)].sum(dtype=torch.int64)) for o in range(0, b.numel(), 1 << 26)))
+
+
+def valid_count(torch, mask, n):
+    if mask is None:
+        return float(n)
+    m = as_bytes(torch, mask)[: (n + 7) // 8]
+    sh = torch.arange(8, device=m.device, dtype=torch.uint8)
+    step = 1 << 24
+    return float(sum(int(((m[o:o + step].unsqueeze(1) >> sh) & 1).reshape(-1)[: n - 8 * o].sum()) for o in range(0, m.numel(), step)))
+
+
+def dump_columns(torch, arrays, prefix, cols, n):
+    """Sampled values and validity of output columns of n rows each, plus whole-column byte sums and valid counts."""
+    idx_np = sample_rows(n)
+    idx = torch.from_numpy(idx_np).cuda()
+    valid, sums, counts = [], [], []
+    for i, c in enumerate(cols):
+        name = f"{prefix}col{i:03d}"
+        if c.dtype.type_id == STRING:
+            arrays[name + "_len"], arrays[name + "_chars"] = gather_lists(torch, c.offsets, c.data, idx)
+        else:
+            arrays[name] = exact_f64(gather_elems(torch, c.data, idx, SIZE[c.dtype.type_id]))
+        sums.append(byte_sum(torch, c.data))
+        m = c.mask.reshape(-1).view(torch.int32) if c.mask is not None else None
+        valid.append(((m[idx >> 5] >> (idx & 31)) & 1).cpu().numpy() if m is not None else np.ones(len(idx_np)))
+        counts.append(valid_count(torch, c.mask, n))
+    arrays[prefix + "sample_rows"] = idx_np.astype(np.float64)
+    arrays[prefix + "validity"] = np.array(valid, dtype=np.float32).reshape(len(cols), len(idx_np))
+    arrays[prefix + "byte_sums"] = np.array(sums, dtype=np.float64)
+    arrays[prefix + "valid_counts"] = np.array(counts, dtype=np.float64)
+
+
+def dump_rows(torch, arrays, prefix, offsets, data, n):
+    """Sampled rows (lengths and bytes) of a buffer of n variable-length rows, plus its byte sum."""
+    idx_np = sample_rows(n)
+    idx = torch.from_numpy(idx_np).cuda()
+    arrays[prefix + "sample_rows"] = idx_np.astype(np.float64)
+    arrays[prefix + "row_len"], arrays[prefix + "row_bytes"] = gather_lists(torch, offsets, data, idx)
+    arrays[prefix + "byte_sum"] = np.array([byte_sum(torch, data)])
+
+
+def write_dump(out_dir, arrays):
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT_BYTES:
+        raise SystemExit(f"bench: --dump-outputs would write {total} bytes (limit {DUMP_LIMIT_BYTES})")
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        assert a.dtype in (np.float32, np.float64), name
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a))
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -341,6 +447,13 @@ def run_ours(args, wl, rank, world):
     if cuprof:
         torch.cuda.cudart().cudaProfilerStop()
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        arrays = {"null_counts": nulls.cpu().numpy().astype(np.float64)}
+        dump_columns(torch, arrays, "", outs, n)
+        if hout is not None:
+            arrays["hash"] = exact_f64(gather_elems(torch, hout, torch.from_numpy(sample_rows(n)).cuda(), 8))
+            arrays["hash_byte_sum"] = np.array([byte_sum(torch, hout)])
+        write_dump(args.dump_outputs, arrays)
     total_ms = t0.elapsed_time(t1)
     kern_ms = float(np.mean([a.elapsed_time(b) for a, b in evs]))
     tt = torch.tensor([total_ms, kern_ms], dtype=torch.float64, device="cuda")
@@ -357,14 +470,6 @@ def run_ours(args, wl, rank, world):
                 "kernel": "srj::from_rows_kernel" + (" + row_hash_stream_kernel over the key columns just written (one C-ABI call)" if wl.get("hash_keys") else ""),
                 "kernel_ms": round(kern_ms, 4), "algorithmic_bytes_per_row": bpr, "rows_per_launch": n,
                 "peak_source": peak_src, "this_box_copy_gbs": box_copy_gbs(torch) if rank == 0 else None}
-    tr = os.path.join(ROOT, "profiles", f"traffic_{args.workload}.json")
-    if os.path.exists(tr):
-        try:
-            j = json.load(open(tr))
-            roofline["traffic"] = j["dram_bytes_per_launch"] * (n / j["rows_per_launch"])
-            roofline["traffic_source"] = j.get("source")
-        except Exception:
-            pass
 
     # ---- multi-GPU config: NCCL all-gather of the per-column chunks over NVLink (north_star) ---------------
     # Each rank contributes the columns of its first n/world rows; every GPU ends with the n-row table.
@@ -439,7 +544,7 @@ def run_ours(args, wl, rank, world):
                 "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_per_step, "higher_is_better": True,
                 "scaling": "weak", "vs_baseline": None, "dtype": "u8", "data": "synthetic",
                 "config": {"workload": wl["name"], "rows_per_gpu": n, "row_bytes": row_size, "columns": len(types),
-                           "l2": "inputs+outputs (%.1f GB) >> 126 MB L2, no flush needed" % (bpr * n / 1e9),
+                           "l2": "inputs+outputs (%.1f GB) >> 50 MB L2, no flush needed" % (bpr * n / 1e9),
                            "launch": "one srj_convert_from_rows_fixed call over all rows (C ABI takes int64 row counts; "
                                      "rows were produced by srj_convert_to_rows in %d <=2GiB batches)" % nbatches,
                            "sharding": "contiguous row range per GPU, no data-path collective"},
@@ -722,6 +827,15 @@ def run_c3(args, wl, rank, world):
         torch.cuda.cudart().cudaProfilerStop()
     ms_gather = timed(True, args.steps) if do_gather else None    # conversion + all-gather, inside the step
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        arrays = {}
+        last = outs[(rounds - 1) % pool]
+        if args.direction == "from_rows":
+            arrays["null_counts"] = nulls.cpu().numpy().astype(np.float64)
+            dump_columns(torch, arrays, "", last["cols"], nb)
+        else:
+            dump_rows(torch, arrays, "", last["offs"], last["data"], nb)
+        write_dump(args.dump_outputs, arrays)
     ms_per_step = ms_gather if do_gather else ms_convert
     rows_step = rounds * nb                                       # rows one rank converts per step
     value = world * rows_step / (ms_per_step * 1e-3)
@@ -732,14 +846,6 @@ def run_c3(args, wl, rank, world):
                 if args.direction == "from_rows" else "whole conversion of a batch (all kernels of the two C-ABI calls)",
                 "algorithmic_bytes_per_row": alg_step / rows_step, "rows_per_launch": nb, "peak_source": peak_src,
                 "ms_per_batch": ms_convert / rounds, "per_gpu": True}
-    tr = os.path.join(ROOT, "profiles", "traffic_c3.json")
-    if os.path.exists(tr) and args.direction == "from_rows":
-        try:
-            j = json.load(open(tr))
-            roofline["traffic"] = j["dram_bytes_per_launch"] * (nb / j["rows_per_launch"])
-            roofline["traffic_source"] = j.get("source")
-        except Exception:
-            pass
     if do_gather:
         sent = slab_bytes
         gms = max(ms_gather - ms_convert, 1e-9) / rounds
@@ -796,7 +902,7 @@ def run_c3(args, wl, rank, world):
                            "resident_pool_batches": pool, "avg_row_bytes": batches[0]["rows"].child.size / nb,
                            "sharding": "contiguous row range per GPU" + (", all-gather inside the timed step" if do_gather else
                                                                          ", no collective (single GPU or --no-gather)"),
-                           "l2": "each batch touches ~%.1f GB >> 126 MB L2; pool of %d distinct batches" % (alg[0] / 1e9, pool)},
+                           "l2": "each batch touches ~%.1f GB >> 50 MB L2; pool of %d distinct batches" % (alg[0] / 1e9, pool)},
                 "hbm_gbs": round(achieved, 1), "roofline": roofline, "cpu_baseline": cpu, "e2e": e2e,
                 "gpu_launches": args.steps * rounds * kernels_per_batch, "clocks": clocks}
         if gather_info:
@@ -916,10 +1022,19 @@ def run_nvbench(args, wl, rank, world):
         times = []
         for _ in range(args.steps):
             t0 = time.perf_counter()
-            fn()
+            last = fn()
             torch.cuda.synchronize()
             times.append(time.perf_counter() - t0)
         res[direction] = float(np.median(times))
+        if args.dump_outputs and direction == args.direction:
+            arrays = {}
+            for j, r in enumerate(last):
+                if direction == "from_rows":
+                    dump_columns(torch, arrays, f"b{j}_", r.columns, r.columns[0].size)
+                else:
+                    dump_rows(torch, arrays, f"b{j}_", r.offsets, r.child.data, r.size)
+            write_dump(args.dump_outputs, arrays)
+        del last
     peak, peak_src = load_peaks()
     sec = res[args.direction]
     print(json.dumps({"metric": "rows_per_sec_convert_" + args.direction, "value": n / sec, "unit": "rows/s", "n_gpus": 1,
@@ -1071,6 +1186,10 @@ def run_partition(args, wl, rank, world):
     e[2].record(stream)
     torch.cuda.synchronize()
     clocks = sampler.stop()
+    if args.dump_outputs:
+        arrays = {"partition_offsets": offs.cpu().numpy().astype(np.float64), "null_counts": nulls.cpu().numpy().astype(np.float64)}
+        dump_columns(torch, arrays, "", outs, n)
+        write_dump(args.dump_outputs, arrays)
     plan_ms = e[0].elapsed_time(e[1]) / args.steps
     ms = e[1].elapsed_time(e[2]) / args.steps
     peak, peak_src = load_peaks()
@@ -1080,7 +1199,7 @@ def run_partition(args, wl, rank, world):
     print(json.dumps({"metric": "rows_per_sec_hash_partition", "value": n / (ms * 1e-3), "unit": "rows/s", "n_gpus": 1, "steps": args.steps,
                       "warmup": args.warmup, "ms_per_step": ms, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
                       "dtype": "u8", "data": "synthetic",
-                      "config": {"workload": wl["name"], "rows": n, "partitions": P, "l2": "inputs 9.6 GB >> 126 MB L2"},
+                      "config": {"workload": wl["name"], "rows": n, "partitions": P, "l2": "inputs 9.6 GB >> 50 MB L2"},
                       "roofline": {"bound": "hbm", "achieved": round(gbs, 1), "peak": peak, "unit": "GB/s", "frac": round(gbs / peak, 4),
                                    "traffic": None, "kernel": "whole step: murmur3 + ids/histogram + scan + ranks + 23 column scatters + 23 mask gathers",
                                    "algorithmic_bytes_per_row": bpr, "peak_source": peak_src, "plan_only_ms": plan_ms},
@@ -1124,12 +1243,19 @@ def run_shuffle(args, wl, rank, world):
         sampler.start()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record(stream)
-    for _ in range(args.steps):
-        step()
+    for s in range(args.steps):
+        if args.dump_outputs and s == args.steps - 1:
+            out = step()
+        else:
+            step()
     e1.record(stream)
     dist.barrier()
     torch.cuda.synchronize()
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        arrays = {}
+        dump_columns(torch, arrays, "", out.columns, out.getRowCount())
+        write_dump(args.dump_outputs, arrays)
     t = torch.tensor([e0.elapsed_time(e1) / args.steps], dtype=torch.float64, device="cuda")
     dist.all_reduce(t, op=dist.ReduceOp.MAX)
     ms = float(t[0])
@@ -1145,7 +1271,7 @@ def run_shuffle(args, wl, rank, world):
                           "vs_baseline": None, "dtype": "u8", "data": "synthetic",
                           "config": {"workload": wl["name"], "rows_per_gpu": n, "partitions": world * k,
                                      "collective": "torch.distributed.all_to_all_single (NCCL) inside the timed step",
-                                     "l2": "every pass touches >= 4.8 GB per GPU >> 126 MB L2"},
+                                     "l2": "every pass touches >= 4.8 GB per GPU >> 50 MB L2"},
                           "roofline": {"bound": "hbm", "achieved": round(gbs, 1), "peak": peak, "unit": "GB/s", "frac": round(gbs / peak, 4),
                                        "traffic": None, "kernel": "whole step per GPU: murmur3 + partition plan + column moves + kudo split + all-to-all + assemble",
                                        "algorithmic_bytes_per_row": bpr, "peak_source": peak_src, "per_gpu": True,
@@ -1206,6 +1332,17 @@ def run_kudo(args, wl, rank, world):
     e1.record(stream)
     torch.cuda.synchronize()
     clocks = sampler.stop()
+    if args.dump_outputs:
+        arrays = {}
+        if args.direction == "from_rows":
+            dump_columns(torch, arrays, "", outs, n)
+        else:
+            arrays["partition_offsets"] = offs.cpu().numpy().astype(np.float64)
+            pos = torch.from_numpy(sample_rows(total.value)).cuda()
+            arrays["buffer_sample_bytes"] = gather_elems(torch, buf, pos, 1)[:, 0].astype(np.float32)
+            arrays["buffer_sample_pos"] = pos.cpu().numpy().astype(np.float64)
+            arrays["buffer_byte_sum"] = np.array([byte_sum(torch, buf)])
+        write_dump(args.dump_outputs, arrays)
     ms = e0.elapsed_time(e1) / args.steps
     peak, peak_src = load_peaks()
     bpr = 2 * (sum(SIZE[t] for t in types) + len(types) / 8.0)     # the table once, the partitions once
@@ -1214,7 +1351,7 @@ def run_kudo(args, wl, rank, world):
     print(json.dumps({"metric": f"rows_per_sec_kudo_{what}", "value": n / (ms * 1e-3), "unit": "rows/s", "n_gpus": 1, "steps": args.steps,
                       "warmup": args.warmup, "ms_per_step": ms, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8",
                       "data": "synthetic", "config": {"workload": wl["name"], "rows": n, "partitions": P, "buffer_bytes": total.value,
-                                                      "l2": "table 9.6 GB + buffer 9.9 GB >> 126 MB L2"},
+                                                      "l2": "table 9.6 GB + buffer 9.9 GB >> 50 MB L2"},
                       "roofline": {"bound": "hbm", "achieved": round(gbs, 1), "peak": peak, "unit": "GB/s", "frac": round(gbs / peak, 4), "traffic": None,
                                    "kernel": f"kudo_{what}_kernel", "algorithmic_bytes_per_row": bpr, "peak_source": peak_src},
                       "cpu_baseline": _cpu_f("kudo_" + what, wl, 4_000_000, P=P), "e2e": None, "gpu_launches": args.steps, "clocks": clocks}))
@@ -1271,6 +1408,17 @@ def run_unsafe(args, wl, rank, world):
     e1.record(stream)
     torch.cuda.synchronize()
     clocks = sampler.stop()
+    if args.dump_outputs:
+        arrays = {}
+        if args.direction == "to_rows":
+            idx_np = sample_rows(n)
+            arrays["sample_rows"] = idx_np.astype(np.float64)
+            arrays["rows"] = exact_f64(gather_elems(torch, rows, torch.from_numpy(idx_np).cuda(), row_bytes))
+            arrays["byte_sum"] = np.array([byte_sum(torch, rows)])
+        else:
+            arrays["null_counts"] = nulls.cpu().numpy().astype(np.float64)
+            dump_columns(torch, arrays, "", outs, n)
+        write_dump(args.dump_outputs, arrays)
     ms = e0.elapsed_time(e1) / args.steps
     peak, peak_src = load_peaks()
     bpr = row_bytes + sum(SIZE[t] for t in types) + len(types) / 8.0
@@ -1279,7 +1427,7 @@ def run_unsafe(args, wl, rank, world):
                       "unit": "rows/s", "n_gpus": 1, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms, "higher_is_better": True,
                       "scaling": "weak", "vs_baseline": None, "dtype": "u8", "data": "synthetic",
                       "config": {"workload": wl["name"], "rows": n, "row_bytes": row_bytes, "direction": args.direction,
-                                 "l2": "rows 13.2 GB + columns 7.2 GB >> 126 MB L2"},
+                                 "l2": "rows 13.2 GB + columns 7.2 GB >> 50 MB L2"},
                       "roofline": {"bound": "hbm", "achieved": round(gbs, 1), "peak": peak, "unit": "GB/s", "frac": round(gbs / peak, 4),
                                    "traffic": None, "kernel": "ur_to_rows_kernel" if args.direction == "to_rows" else "ur_from_rows_kernel",
                                    "algorithmic_bytes_per_row": bpr, "peak_source": peak_src},
@@ -1370,7 +1518,13 @@ def main():
     ap.add_argument("--no-gather", action="store_true", help="multi-GPU: skip the all-gather (conversion-only scaling)")
     ap.add_argument("--gather", default="p2p", choices=["p2p", "nccl"],
                     help="multi-GPU all-gather transport: copy engines over NVLink peer memory (default) or ncclAllGather")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last step computed as DIR/<name>.npy (float32/float64, <= 64 MB)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs dumps the GPU path (--impl ours)")
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     rank = int(os.environ.get("RANK", 0))
     world = int(os.environ.get("WORLD_SIZE", 1))

@@ -1,5 +1,5 @@
 /*
- * srj_b200.h -- C ABI of libsrj_b200.so: the B200-native (sm_100a) replacement for the
+ * srj_b200.h -- C ABI of libsrj_b200.so: the H100-native (sm_90a) replacement for the
  * row<->columnar + Spark row-hash hot path of NVIDIA/spark-rapids-jni.
  *
  * This is the drop-in boundary (SURVEY.md 8b).  Every entry point below is what the reference's

@@ -1,6 +1,6 @@
 """CPU restatement of the reference's Kudo shuffle wire format for FLAT tables -- TEST INFRASTRUCTURE ONLY.
 
-Follows (file:line in /root/reference/src/main/java/com/nvidia/spark/rapids/jni/kudo/):
+Follows (file:line in the reference repository's src/main/java/com/nvidia/spark/rapids/jni/kudo/):
   KudoSerializer.java:49-171        the format: header | validity | offsets | data
   KudoTableHeader.java:42,186-200   header = "KUD0" (0x4B554430), offset, numRows, validityBufferLen, offsetBufferLen,
                                     totalDataLen, numColumns -- seven BIG-ENDIAN ints -- then the hasValidity bitset,

@@ -18,7 +18,7 @@
  *     round-trip identity.
  *
  * Every function cites the reference file:line it follows.  Paths are relative to
- * /root/reference; RC = src/main/cpp/src/row_conversion.cu.
+ * the reference repository's root; RC = src/main/cpp/src/row_conversion.cu.
  */
 #include <stdint.h>
 #include <stddef.h>

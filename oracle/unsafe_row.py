@@ -1,6 +1,6 @@
 """CPU restatement of Apache Spark's UnsafeRow format -- TEST INFRASTRUCTURE ONLY (tests/, smoke(), bench cpu legs).
 
-PARITY UNPINNED: /root/reference holds no vector of this format (the reference speaks JCUDF rows only,
+PARITY UNPINNED: the reference repository holds no vector of this format (the reference speaks JCUDF rows only,
 RowConversion.java:44-117; the plugin adapts them with CudfUnsafeRow).  The format is Apache Spark's, restated from its
 published sources (branch-3.5):
   sql/catalyst/src/main/java/org/apache/spark/sql/catalyst/expressions/UnsafeRow.java

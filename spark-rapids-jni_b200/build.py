@@ -1,4 +1,4 @@
-"""Builds libsrj_b200.so (hand-written sm_100a CUDA + the C ABI) in-tree with nvcc.
+"""Builds libsrj_b200.so (hand-written sm_90a CUDA + the C ABI) in-tree with nvcc.
 
     python spark-rapids-jni_b200/build.py [--force] [--verbose]
 
@@ -17,7 +17,7 @@ OUT = os.path.join(HERE, "srj_b200", "libsrj_b200.so")
 SOURCES = ["capi.cu", "from_rows.cu", "from_rows_wide.cu", "to_rows.cu", "to_rows_var.cu", "strings.cu", "hash.cu", "hash_nested.cu", "sharding.cu", "partition.cu", "unsafe_row.cu", "kudo.cu", "host_api.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--shared", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "-ccbin", "/usr/bin/g++",
     "--expt-relaxed-constexpr", "-Xptxas", "-v" if os.environ.get("SRJ_PTXAS_V") else "-O3",
 ]
@@ -55,7 +55,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         failed |= p.returncode != 0
     if failed:
         raise RuntimeError("nvcc failed")
-    cmd = [NVCC, "--shared", "-gencode", "arch=compute_100a,code=sm_100a", "-ccbin", "/usr/bin/g++", "-Xlinker", "--no-undefined", "-o", OUT] + objs
+    cmd = [NVCC, "--shared", "-gencode", "arch=compute_90a,code=sm_90a", "-ccbin", "/usr/bin/g++", "-Xlinker", "--no-undefined", "-o", OUT] + objs
     subprocess.check_call(cmd)
     return OUT
 

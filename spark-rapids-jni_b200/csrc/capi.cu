@@ -40,6 +40,14 @@ int cuda_fail(cudaError_t e, const char* what)
   return e == cudaErrorMemoryAllocation ? SRJ_ENOMEM : SRJ_ECUDA;
 }
 
+int sm_count()
+{
+  int dev = 0, nsm = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+    return 132;  // H100 SXM; a failing device surfaces at the launch that follows
+  return nsm;
+}
+
 static int size_of_type(int32_t t)
 {
   switch (t) {
@@ -160,7 +168,7 @@ using namespace srj;
 
 extern "C" {
 
-const char* srj_version(void) { return "srj_b200 0.1.0 (sm_100a)"; }
+const char* srj_version(void) { return "srj_b200 0.1.0 (sm_90a)"; }
 const char* srj_last_error(void) { return g_err; }
 const char* srj_status_string(int s)
 {
@@ -229,12 +237,11 @@ int srj_plan_create(const int32_t* type_ids, const int32_t* scales, int32_t num_
   p->fr_class_begin[kNumClasses] = static_cast<int32_t>(p->fr_entries.size());
   p->tr_class_begin[kNumClasses] = static_cast<int32_t>(p->tr_entries.size());
 
-  // from_rows tiling (shared memory budget 227 KB/CTA on sm_100)
+  // from_rows tiling (shared memory budget 227 KB/CTA on sm_90)
   Tiling& tl = p->tiling;
   const int S = p->fixed_row_size;
   // Narrow rows (512 rows fit 64 KB): three 64 KB stages.  Wider rows: two 100 KB stages -- taller tiles mean longer
-  // contiguous pieces per column and per CTA, which is what the DRAM likes once the part is warm (C2, 200 B rows:
-  // 256-row tiles 92.3 %, 512-row tiles 94.7 % of the measured copy bandwidth on the same box).
+  // contiguous pieces per column and per CTA, which is what the DRAM likes once the part is warm.
   if (S <= 128) { tl.num_stages = 3; tl.stage_bytes = 64 * 1024; }
   else          { tl.num_stages = 2; tl.stage_bytes = 100 * 1024; }
   int fitrows = tl.stage_bytes / S;

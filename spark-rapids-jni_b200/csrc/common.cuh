@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for the sm_100a row<->column kernels:
+// common.cuh -- shared device helpers for the sm_90a row<->column kernels:
 // mbarrier / TMA (1-D bulk async copy) PTX wrappers, warp utilities, error plumbing.
 #pragma once
 #include <cuda_runtime.h>
@@ -13,6 +13,7 @@ constexpr int kWarp = 32;
 // ---- error plumbing (host) --------------------------------------------------------------------
 void set_error(const char* fmt, ...);
 int cuda_fail(cudaError_t e, const char* what);
+int sm_count();  // multiprocessors of the current device (grid caps of the grid-stride kernels)
 #define SRJ_CUDA_TRY(expr)                                     \
   do {                                                         \
     cudaError_t _e = (expr);                                   \
@@ -73,7 +74,7 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity)
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity)
 {
   while (!mbar_try_wait(bar, parity)) {}  // try_wait suspends in hardware up to the hint; no software back-off
-                                          // (a __nanosleep here cost 4% on C2: slower wake-up)
+                                          // (a __nanosleep here wakes up later)
 }
 
 // Waiter that backs off between probes: for issue-bound kernels whose consumer warps finish unevenly

@@ -517,7 +517,7 @@ __device__ __noinline__ void producer_loop(const ProducerArgs p)
   {
     // Super-tiles (a few tiles of consecutive rows) are dealt round-robin to the CTAs, so at any moment
     // the whole grid streams through one contiguous window of the row buffer and of every column --
-    // the access pattern of a plain copy kernel -- instead of 148 far-apart ranges.
+    // the access pattern of a plain copy kernel -- instead of one far-apart range per SM.
     int64_t sup = blockIdx.x;
     int64_t r   = sup * p.super_rows;
     int64_t c1  = tmin(p.num_rows, r + p.super_rows);
@@ -544,7 +544,7 @@ __device__ __noinline__ void producer_loop(const ProducerArgs p)
       } else {
         // load off[r .. r+rows] (coalesced) and pick the largest multiple-of-8 row count that fits.  All the loads
         // are issued before the first use: one memory round trip per tile, not one per 32 rows (a 512-row tile of
-        // a narrow table spent 10 us here, 7x the time its consumers need).
+        // a narrow table spends several times longer here than its consumers need).
         constexpr int kMaxChunks = 17;  // tile_rows <= 512 -> rows + 1 <= 513 offsets
         rows = tmin(rows, 512);
         int32_t ov[kMaxChunks];
@@ -897,7 +897,7 @@ int launch_from_rows(const srj_plan* plan, const uint8_t* rows, const int32_t* r
   SRJ_CUDA_TRY(cudaGetDevice(&dev));
   SRJ_CUDA_TRY(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
   // super-tile = a multiple of the tile height (=> of 32 or 8|16: mask-byte aligned).  Fixed-stride
-  // tables: two tiles (measured: 1 -> 2 tiles +1.5 % on C2, flat beyond).  Variable-width tables cut tiles adaptively inside a
+  // tables: two tiles (faster than one, flat beyond).  Variable-width tables cut tiles adaptively inside a
   // super-tile of >= 4 tiles so the last, shorter tile of a super-tile is amortised.
   const int sup_tiles_env = SRJ_KNOB("SRJ_FR_SUPER", 0);
   const int64_t T  = p.tile_rows;
@@ -912,7 +912,7 @@ int launch_from_rows(const srj_plan* plan, const uint8_t* rows, const int32_t* r
   switch (variant) {
     case 2: rc = launch_variant<7>(p, static_cast<unsigned>(grid), smem, stream); break;
     // 11 consumer warps: 384 threads x 168 registers fills the register file with no spills (15 warps cap
-    // the kernel at 128 registers and spill inside the transpose loop: 76% vs 95% of HBM peak on C2)
+    // the kernel at 128 registers and spill inside the transpose loop)
     default: rc = launch_variant<11>(p, static_cast<unsigned>(grid), smem, stream); break;
   }
   if (rc != SRJ_OK) return rc;

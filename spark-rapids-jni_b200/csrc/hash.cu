@@ -94,8 +94,8 @@ __device__ __forceinline__ void fetch_column(const HashCol& col, const int64_t (
 }
 
 // Each thread makes one pass (load 4 rows of every key column, hash, store), so the kernel lives on occupancy:
-// 4 resident CTAs (64 registers) for the multiply-heavy xxhash64 / murmur3, 5 (48 registers) for hive.  Measured on
-// 100 M rows x (INT32, INT64): xxhash64 1.26 -> 0.99 ms against the unbounded 80-register build.
+// 4 resident CTAs (64 registers) for the multiply-heavy xxhash64 / murmur3, 5 (48 registers) for hive, rather than
+// the unbounded 80-register build.
 template <int KIND>
 __global__ void __launch_bounds__(kHashThreads, KIND == SRJ_HASH_HIVE ? 5 : 4) row_hash_kernel(const __grid_constant__ HashParams p)
 {
@@ -241,7 +241,7 @@ __global__ void __launch_bounds__(kHashThreads, KIND == SRJ_HASH_HIVE ? 5 : 4) r
 // --------------------------------------------------------------------------------------------------
 // Streaming row hash for fixed-width keys (the shuffle-partitioning case: a few 4/8-byte key columns, 10^8 rows).
 // The kernels above issue their global loads from the hashing threads, so every row block waits a DRAM round trip
-// before its multiply chains can start (ncu: long-scoreboard 10 stalls per issue, 37 % of the HBM peak).  Here the
+// before its multiply chains can start (long-scoreboard stalls dominate).  Here the
 // loads are decoupled from the arithmetic, the way the conversion kernels do it:
 //   producer warp : per chunk of kHsRows rows, one TMA bulk copy per key column (a contiguous, 16-byte aligned piece
 //                   of the column) and per mask into a ring of shared-memory stages guarded by full/empty mbarriers;
@@ -498,11 +498,10 @@ int launch_hash(int kind, const srj_column* cols, int32_t num_columns, int64_t n
       int dev = 0, nsm = 0;
       SRJ_CUDA_TRY(cudaGetDevice(&dev));
       SRJ_CUDA_TRY(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
-      // grid = resident CTAs per SM (occupancy) x rounds.  Measured on 100 M rows x (INT32, INT64): the multiply-heavy
-      // kernels like 4 rounds (xxhash64 0.87 -> 0.83 ms, murmur3 0.78 -> 0.74 ms against one CTA per row block),
-      // hive -- pure streaming -- exactly one (0.67 -> 0.63 ms); a grid that is not a multiple of the resident count
-      // leaves a straggler CTA per SM (xxhash64 1.17 ms).
-      static int occ_cache[4] = {0, 0, 0, 0};  // per hash kind; the same for every sm_100a device (benign race)
+      // grid = resident CTAs per SM (occupancy) x rounds: the multiply-heavy kernels take 4 rounds rather than one CTA
+      // per row block, hive -- pure streaming -- exactly one; a grid that is not a multiple of the resident count
+      // leaves a straggler CTA per SM.
+      static int occ_cache[4] = {0, 0, 0, 0};  // per hash kind; the same for every sm_90a device (benign race)
       int occ = occ_cache[kind & 3];
       if (occ == 0) {
         if (kind == SRJ_HASH_XXHASH64)

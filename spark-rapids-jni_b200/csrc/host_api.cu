@@ -81,8 +81,8 @@ int from_rows_host_fixed(const srj_plan* plan, ArenaLease& L, const uint8_t* h_r
   const int nc    = plan->num_columns;
   const int64_t S = plan->fixed_row_size;
   if (chunk_rows <= 0) {
-    // ~1/12 of the input per chunk, between 32 MB and 1 GB of rows (measured on C2: 64 MB chunks 153 M rows/s,
-    // 256 MB 217 M, 1 GB 238 M): per chunk the copies have a fixed cost and the first H2D / last D2H are not overlapped
+    // ~1/12 of the input per chunk, between 32 MB and 1 GB of rows (larger chunks are faster): per chunk the copies
+    // have a fixed cost and the first H2D / last D2H are not overlapped
     int64_t cbytes = std::min<int64_t>(1ll << 30, std::max<int64_t>(32ll << 20, num_rows * S / 12));
     if (const int mb = SRJ_KNOB("SRJ_HOST_CHUNK_MB", 0)) cbytes = static_cast<int64_t>(mb) << 20;
     chunk_rows = std::max<int64_t>(32 * 1024, cbytes / S);

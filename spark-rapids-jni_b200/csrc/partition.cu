@@ -544,7 +544,7 @@ int launch_partition_move_tiles(const srj_column* in, const srj_column* out, con
 
 static unsigned grid_for(int64_t n, int per_block)
 {
-  return static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>((n + per_block - 1) / per_block, 148 * 16)));
+  return static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>((n + per_block - 1) / per_block, int64_t{sm_count()} * 16)));
 }
 
 int launch_partition_scatter_fixed(const void* in, void* out, int elem_size, const int32_t* d_scatter_map, int64_t n, cudaStream_t stream)

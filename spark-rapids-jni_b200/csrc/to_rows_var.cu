@@ -37,7 +37,7 @@ namespace srj {
 
 constexpr int kT3MaxBlocks = 48;    // string blocks per row
 constexpr int kT3MaxItems  = 1024;
-constexpr int kHoist       = 2;     // STRING columns of a block whose offsets are fetched together (1 -> 2: +1.3 %; 4 spills)
+constexpr int kHoist       = 2;     // STRING columns of a block whose offsets are fetched together (4 spills)
 
 struct ToRows3Params {
   const void* const* col_data;

@@ -16,7 +16,7 @@
 //         (offset << 32) | number of bytes, or (offset << 32) | 0 with the null bit set for a NULL.
 //   Rows are a multiple of 8 bytes; variable-length entries follow in field order.  Floating-point payloads are copied
 //   bit for bit (like the reference's row conversion, which moves bytes).
-// No vector of this format exists under /root/reference: parity is pinned on hand-derived known answers of the rules
+// No vector of this format exists in the reference repository: parity is pinned on hand-derived known answers of the rules
 // above (the CPU restatement and its known-answer tests live with the test infrastructure) -- "parity unpinned".
 //
 // Kernels (lane = row: column accesses coalesced, row accesses strided but sector-local -- a thread walks its row):
@@ -328,7 +328,7 @@ static int ur_stage(const int32_t* d_row_offsets, int fixed_row_bytes)
   return std::min(kUrStage, (32 * fixed_row_bytes + 15) & ~15);
 }
 
-static unsigned ur_grid(int64_t n) { return static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, 148 * 8))); }
+static unsigned ur_grid(int64_t n) { return static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, int64_t{sm_count()} * 8))); }
 
 // ---- host side -------------------------------------------------------------------------------------------------------------
 static bool ur_classify(int32_t type_id, int32_t* kind, int32_t* width, int32_t* sext)
@@ -471,7 +471,7 @@ int launch_unsafe_from_rows_strings(const srj_column* out, int32_t ncols, int64_
   const int rc = unsafe_row_layout(types, ncols, &bitset, &fixed, &ndec, &nstr);
   if (rc != SRJ_OK) return rc;
   if (n == 0) return SRJ_OK;
-  const unsigned grid = static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, 148 * 16)));
+  const unsigned grid = static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, int64_t{sm_count()} * 16)));
   for (int c = 0; c < ncols; ++c) {
     if (out[c].type_id != SRJ_STRING) continue;
     ur_chars_kernel<<<grid, 256, 0, stream>>>(rows, d_row_offsets, fixed + 16 * ndec, n, bitset + 8 * c, c >> 6, c & 63, out[c].offsets,

@@ -1,6 +1,6 @@
 """Golden hash vectors transcribed (as DATA) from the reference's own tests.
 
-Sources (paths relative to /root/reference):
+Sources (paths relative to the reference repository's root):
   CPP  = src/main/cpp/tests/hash.cpp
   JAVA = src/test/java/com/nvidia/spark/rapids/jni/HashTest.java
 The expected values there were produced by Apache Spark (see the Scala snippets in CPP:201-266,
