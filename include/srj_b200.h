@@ -220,6 +220,33 @@ SRJ_API int srj_murmur_hash3_32(const srj_column* cols, int32_t num_columns, int
 SRJ_API int srj_hive_hash(const srj_column* cols, int32_t num_columns, int64_t num_rows, int32_t* out,
                           void* stream);
 
+/* ---- SHA-2 of a STRING column, nulls preserved: Hash.sha{224,256,384,512}NullsPreserved, hash/sha.cpp:31-49 ----------
+ * FIPS 180-4 SHA-224 / SHA-256 / SHA-384 / SHA-512 of each row's bytes as lowercase hex: 56 / 64 / 96 / 128 chars per
+ * valid row (the empty string hashes normally).  A null row gives a null output row of zero length; the output mask equals
+ * the input's.  Two steps, like the other STRING outputs:
+ *   srj_sha2_workspace_bytes : bytes of the sizes call's workspace (needed only when the input has a null mask).
+ *   srj_sha2_sizes           : d_out_offsets[rows + 1] of the output and *total_chars (host).  Without an input mask the
+ *                              offsets are width x row and the call does not synchronise; with one it scans the mask
+ *                              and reads the valid count back (one stream synchronisation).  SRJ_EOVERFLOW when the chars
+ *                              would exceed INT32_MAX (nothing is written then).
+ *   srj_sha2_hash            : (async) writes the chars into out->data (16-byte aligned; may be NULL only when
+ *                              *total_chars was 0) at out->offsets (the sizes call's output), and copies the input mask to
+ *                              out->null_mask when out has one (all valid when the input has none).  An input with a
+ *                              mask needs an output mask.
+ * digest_bits is 224, 256, 384 or 512 (else SRJ_EINVAL); the input must be one STRING column (else SRJ_EUNSUPPORTED),
+ * <= INT32_MAX rows.  The output null count equals the input's.
+ */
+SRJ_API int64_t srj_sha2_workspace_bytes(int64_t num_rows);
+SRJ_API int srj_sha2_sizes(int32_t digest_bits, const srj_column* input, int32_t* d_out_offsets, int64_t* total_chars, void* workspace,
+                           void* stream);
+SRJ_API int srj_sha2_hash(int32_t digest_bits, const srj_column* input, const srj_column* out, void* stream);
+
+/* ---- Hash.hostCrc32, hash/HashJni.cpp:143-157: zlib crc32 on the HOST ------------------------------------------------
+ * *out = crc32(crc, buf[0 .. len)), equal to zlib's crc32 and java.util.zip.CRC32, chaining from a previous value.
+ * buf may be NULL only when len == 0; len < 0 or a NULL buffer with len > 0 is SRJ_EINVAL.  Touches no device.
+ */
+SRJ_API int srj_host_crc32(uint32_t crc, const void* buf, int64_t len, uint32_t* out);
+
 /* ---- multi-GPU configuration (SURVEY 8e: row-range shards + one all-gather of per-column chunks) ---------------- */
 /* ---- Spark HashPartitioning on the device (SURVEY 8f rank 1) ---------------------------------------------------
  * The consumer of Hash.murmurHash32: GpuHashPartitioning computes pmod(murmur3_32(42, keys), P) per row and then

@@ -661,6 +661,83 @@ int srj_hive_hash(const srj_column* cols, int32_t num_columns, int64_t num_rows,
 }
 
 // ---------------------------------------------------------------------------------------------------
+// SHA-2 with nulls preserved (sha2.cu) and the host CRC32
+// ---------------------------------------------------------------------------------------------------
+int64_t srj_sha2_workspace_bytes(int64_t num_rows) { return sha2_workspace_bytes(std::max<int64_t>(0, num_rows)); }
+
+static int sha2_check(const char* what, int32_t digest_bits, const srj_column* in)
+{
+  if (sha2_hex_width(digest_bits) == 0) { set_error("%s: digest_bits %d is not one of 224, 256, 384, 512", what, digest_bits); return SRJ_EINVAL; }
+  if (!in) { set_error("%s: input is null", what); return SRJ_EINVAL; }
+  if (in->type_id != SRJ_STRING) { set_error("%s: SHA-2 hashing requires a string column (type id %d)", what, in->type_id); return SRJ_EUNSUPPORTED; }
+  if (in->size < 0 || in->size > INT32_MAX) { set_error("%s: %lld rows", what, static_cast<long long>(in->size)); return SRJ_EINVAL; }
+  if (in->size > 0 && !in->offsets) { set_error("%s: the STRING column has no offsets", what); return SRJ_EINVAL; }
+  return SRJ_OK;
+}
+
+int srj_sha2_sizes(int32_t digest_bits, const srj_column* input, int32_t* d_out_offsets, int64_t* total_chars, void* workspace, void* stream)
+{
+  SRJ_API_RANGE();
+  int rc = sha2_check("sha2_sizes", digest_bits, input);
+  if (rc != SRJ_OK) return rc;
+  if (!d_out_offsets || !total_chars) { set_error("sha2_sizes: bad argument"); return SRJ_EINVAL; }
+  if (input->null_mask && input->size > 0 && !workspace) { set_error("sha2_sizes: an input with a null mask needs the workspace (srj_sha2_workspace_bytes)"); return SRJ_EINVAL; }
+  rc = launch_sha2_sizes(digest_bits, *input, d_out_offsets, total_chars, workspace, static_cast<cudaStream_t>(stream));
+  if (rc == SRJ_EOVERFLOW)
+    set_error("sha2_sizes: %lld chars of SHA-%d hex exceed one STRING column (INT32_MAX): hash fewer rows per call", static_cast<long long>(*total_chars), digest_bits);
+  return rc;
+}
+
+int srj_sha2_hash(int32_t digest_bits, const srj_column* input, const srj_column* out, void* stream)
+{
+  SRJ_API_RANGE();
+  int rc = sha2_check("sha2_hash", digest_bits, input);
+  if (rc != SRJ_OK) return rc;
+  if (!out || out->size != input->size || (input->size > 0 && !out->offsets)) { set_error("sha2_hash: the output needs the offsets of srj_sha2_sizes and the input's row count"); return SRJ_EINVAL; }
+  if (input->null_mask && !out->null_mask && input->size > 0) { set_error("sha2_hash: the input has a null mask but the output has none"); return SRJ_EINVAL; }
+  if (!input->null_mask && input->size > 0 && !out->data) { set_error("sha2_hash: the output has no chars buffer"); return SRJ_EINVAL; }
+  if (reinterpret_cast<uintptr_t>(out->data) & 15) { set_error("sha2_hash: the output chars must be 16-byte aligned"); return SRJ_EINVAL; }
+  return launch_sha2(digest_bits, *input, *out, static_cast<cudaStream_t>(stream));
+}
+
+// zlib's crc32 (reflected polynomial 0xEDB88320), slicing by 8: eight 256-entry tables, eight input bytes per step.
+namespace {
+struct Crc32Tables {
+  uint32_t t[8][256];
+  Crc32Tables()
+  {
+    for (uint32_t i = 0; i < 256; ++i) {
+      uint32_t c = i;
+      for (int k = 0; k < 8; ++k) c = (c & 1) ? 0xEDB88320u ^ (c >> 1) : c >> 1;
+      t[0][i] = c;
+    }
+    for (int s = 1; s < 8; ++s)
+      for (int i = 0; i < 256; ++i) t[s][i] = (t[s - 1][i] >> 8) ^ t[0][t[s - 1][i] & 0xff];
+  }
+};
+}  // namespace
+
+int srj_host_crc32(uint32_t crc, const void* buf, int64_t len, uint32_t* out)
+{
+  SRJ_API_RANGE();
+  if (!out || len < 0 || (!buf && len > 0)) { set_error("host_crc32: len must be >= 0, and the buffer may be NULL only when len is 0"); return SRJ_EINVAL; }
+  static const Crc32Tables T;   // built once, thread-safe (function-local static)
+  const auto* p = static_cast<const uint8_t*>(buf);
+  uint32_t c    = ~crc;
+  for (; len >= 8; len -= 8, p += 8) {   // little-endian host: the low word holds the first four bytes
+    uint32_t lo, hi;
+    memcpy(&lo, p, 4);
+    memcpy(&hi, p + 4, 4);
+    lo ^= c;
+    c = T.t[7][lo & 0xff] ^ T.t[6][(lo >> 8) & 0xff] ^ T.t[5][(lo >> 16) & 0xff] ^ T.t[4][lo >> 24] ^ T.t[3][hi & 0xff] ^
+        T.t[2][(hi >> 8) & 0xff] ^ T.t[1][(hi >> 16) & 0xff] ^ T.t[0][hi >> 24];
+  }
+  for (; len > 0; --len, ++p) c = T.t[0][(c ^ *p) & 0xff] ^ (c >> 8);
+  *out = ~c;
+  return SRJ_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
 // Spark HashPartitioning: pmod(murmur3_32(seed, keys), P) + stable partition (partition.cu)
 // ---------------------------------------------------------------------------------------------------
 int64_t srj_partition_workspace_bytes(int64_t num_rows, int32_t num_partitions)

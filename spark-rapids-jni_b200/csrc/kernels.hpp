@@ -100,6 +100,13 @@ int launch_unsafe_from_rows(const srj_column* out, int32_t ncols, int64_t n, con
 int launch_unsafe_from_rows_strings(const srj_column* out, int32_t ncols, int64_t n, const uint8_t* rows, const int32_t* d_row_offsets,
                                     cudaStream_t stream);
 
+// ---- sha2.cu: SHA-224/256/384/512 of a STRING column as lowercase hex, nulls preserved ----
+int32_t sha2_hex_width(int32_t digest_bits);    // hex chars per valid row, 0 for an unknown digest
+int64_t sha2_workspace_bytes(int64_t n);
+// output offsets (width x valid rows before each row) and, on the host, the chars total; SRJ_EOVERFLOW beyond INT32_MAX
+int launch_sha2_sizes(int32_t digest_bits, const srj_column& in, int32_t* d_offsets, int64_t* h_total, void* workspace, cudaStream_t stream);
+int launch_sha2(int32_t digest_bits, const srj_column& in, const srj_column& out, cudaStream_t stream);
+
 // ---- kudo.cu: the Kudo shuffle wire format for flat tables (split / assemble) ----
 int64_t kudo_workspace_bytes(int32_t ncols, int32_t P);
 int launch_kudo_split_sizes(const srj_column* cols, int32_t ncols, const int32_t* d_splits, int32_t P, int64_t* d_part_offsets, int64_t* h_total,

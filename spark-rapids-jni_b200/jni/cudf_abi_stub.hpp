@@ -35,6 +35,7 @@ struct column_view {
   size_type size() const;
   size_type offset() const;
   size_type num_children() const;
+  size_type null_count() const;
   column_view child(size_type i) const;
   bitmask_type const* null_mask() const;
   template <typename T> T const* head() const;     // base pointer, offset not applied

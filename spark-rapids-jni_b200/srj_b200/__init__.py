@@ -13,6 +13,8 @@ would (INTEGRATION.md).  torch is used for device memory and streams only.
   Hash.murmurHash32(seed, columns) / Hash.murmurHash32(columns)   Hash.java:34-62
   Hash.xxhash64(seed, columns) / Hash.xxhash64(columns)           Hash.java:64-89
   Hash.hiveHash(columns)                                           Hash.java:91-105
+  Hash.sha{224,256,384,512}NullsPreserved(column)                  Hash.java:107-162
+  Hash.hostCrc32(crc, buffer)                                      Hash.java:164-174
 """
 from __future__ import annotations
 
@@ -470,3 +472,62 @@ class Hash:
             out = _empty(n, torch.int32, dev)
             N.check(N.lib().srj_hive_hash(_carray(cols), len(cols), n, out.data_ptr(), _stream_ptr()), "hiveHash")
             return ColumnVector(DType.INT32, n, out.view(torch.uint8), None, null_count=0)
+
+    # ---- SHA-2 with nulls preserved (Hash.java:107-162) and hostCrc32 (Hash.java:164-174)
+    @staticmethod
+    def _sha2(column: ColumnView, digest_bits: int) -> ColumnVector:
+        """STRING column -> STRING column of lowercase hex SHA-2 digests; null rows stay null (zero length)."""
+        if column is None:
+            raise ValueError("SHA-2 hashing requires a non-null column")            # IllegalArgumentException, Hash.java:108-110
+        if column.dtype.type_id != DType.STRING:
+            raise ValueError("SHA-2 hashing requires a string column")              # Hash.java:111-113
+        n = column.size
+        dev = next((t.device for t in (column.offsets, column.data, column.mask) if t is not None),
+                   torch.device("cuda", torch.cuda.current_device()))
+        with torch.cuda.device(dev):
+            lib = N.lib()
+            stream = _stream_ptr()
+            cin = column._c()
+            offsets = _empty(n + 1, torch.int32, dev)
+            ws = None
+            if column.mask is not None and n > 0:
+                ws = _empty(max(lib.srj_sha2_workspace_bytes(n), 8), torch.uint8, dev)   # rmm allocation in the JNI shim
+            total = C.c_int64(0)
+            N.check(lib.srj_sha2_sizes(digest_bits, C.byref(cin), offsets.data_ptr(), C.byref(total),
+                                       ws.data_ptr() if ws is not None else None, stream), f"sha{digest_bits}NullsPreserved")
+            chars = _empty(total.value, torch.uint8, dev)
+            mask = _empty((n + 31) // 32, torch.int32, dev) if column.mask is not None else None
+            out = ColumnVector(DType.STRING, n, chars, mask, offsets, null_count=column.getNullCount())
+            cout = out._c()
+            N.check(lib.srj_sha2_hash(digest_bits, C.byref(cin), C.byref(cout), stream), f"sha{digest_bits}NullsPreserved")
+            return out
+
+    @staticmethod
+    def sha224NullsPreserved(column: ColumnView) -> ColumnVector:
+        return Hash._sha2(column, 224)
+
+    @staticmethod
+    def sha256NullsPreserved(column: ColumnView) -> ColumnVector:
+        return Hash._sha2(column, 256)
+
+    @staticmethod
+    def sha384NullsPreserved(column: ColumnView) -> ColumnVector:
+        return Hash._sha2(column, 384)
+
+    @staticmethod
+    def sha512NullsPreserved(column: ColumnView) -> ColumnVector:
+        return Hash._sha2(column, 512)
+
+    @staticmethod
+    def hostCrc32(crc: int, buffer) -> int:
+        """zlib crc32 of a host buffer (bytes-like, numpy array or CPU tensor), continuing from `crc`."""
+        if isinstance(buffer, torch.Tensor):
+            if buffer.is_cuda:
+                raise ValueError("hostCrc32 takes a host buffer")
+            buffer = buffer.contiguous().numpy()
+        arr = np.frombuffer(buffer, dtype=np.uint8) if not isinstance(buffer, np.ndarray) else \
+            np.ascontiguousarray(buffer).reshape(-1).view(np.uint8)
+        out = C.c_uint32(0)
+        N.check(N.lib().srj_host_crc32(C.c_uint32(int(crc) & 0xFFFFFFFF), arr.ctypes.data_as(C.c_void_p) if arr.size else None,
+                                       arr.size, C.byref(out)), "hostCrc32")
+        return out.value

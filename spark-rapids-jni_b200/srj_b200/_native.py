@@ -64,6 +64,10 @@ SYMBOLS = {
     "srj_murmur_hash3_32": (C.c_int, [C.POINTER(SrjColumn), C.c_int32, C.c_int64, C.c_uint32, C.c_void_p,
                                       C.c_void_p]),
     "srj_hive_hash": (C.c_int, [C.POINTER(SrjColumn), C.c_int32, C.c_int64, C.c_void_p, C.c_void_p]),
+    "srj_sha2_workspace_bytes": (C.c_int64, [C.c_int64]),
+    "srj_sha2_sizes": (C.c_int, [C.c_int32, C.POINTER(SrjColumn), C.c_void_p, C.POINTER(C.c_int64), C.c_void_p, C.c_void_p]),
+    "srj_sha2_hash": (C.c_int, [C.c_int32, C.POINTER(SrjColumn), C.POINTER(SrjColumn), C.c_void_p]),
+    "srj_host_crc32": (C.c_int, [C.c_uint32, C.c_void_p, C.c_int64, C.POINTER(C.c_uint32)]),
     "srj_partition_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int32]),
     "srj_hash_partition": (C.c_int, [C.POINTER(SrjColumn), C.c_int32, C.c_int64, C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
