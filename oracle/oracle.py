@@ -305,13 +305,25 @@ def nested_hash(kind: str, cols: Sequence[HCol], seed: int = 0) -> np.ndarray:
             cache[id(c)] = _leaf_c(c)
         return C.cast(cache[id(c)][0], C.c_void_p)
 
+    # xxhash64 does not look at LIST / STRUCT level nulls (xxhash64.cu:460-462).  murmur3 hashes the table the cudf row
+    # hasher prepared (murmur_hash.cu:210): struct nulls pushed down into the fields and null list rows emptied
+    # (cudf row_operators.cu:845-852, structs/utilities.cu:617-633), so a null LIST or STRUCT element contributes nothing.
+    def live(c, i):
+        return kind == "xxhash64" or c.mask is None or bool((int(c.mask[i >> 5]) >> (i & 31)) & 1)
+
     def chain(c, lo, hi, h):                       # xxhash64 / murmur3: depth-first over the leaves of [lo, hi)
         if c.type_id == LIST:
-            return chain(c.children[0], int(c.offsets[lo]), int(c.offsets[hi]), h)
+            if kind == "xxhash64" or c.mask is None:
+                return chain(c.children[0], int(c.offsets[lo]), int(c.offsets[hi]), h)
+            for i in range(lo, hi):
+                if live(c, i):
+                    h = chain(c.children[0], int(c.offsets[i]), int(c.offsets[i + 1]), h)
+            return h
         if c.type_id == STRUCT:
             for i in range(lo, hi):
-                for f in c.children:
-                    h = chain(f, i, i + 1, h)
+                if live(c, i):
+                    for f in c.children:
+                        h = chain(f, i, i + 1, h)
             return h
         for i in range(lo, hi):
             h = L.orc_xx_elem(cptr(c), i, h) if kind == "xxhash64" else L.orc_mm_elem(cptr(c), i, h)
@@ -390,7 +402,7 @@ def spark_pmod(h: np.ndarray, n: int) -> np.ndarray:
 def partition_ids(keys: Sequence[HCol], num_partitions: int, seed: int = 42) -> np.ndarray:
     """GpuHashPartitioning: pmod(murmur3_32(seed, keys), numPartitions)."""
     nested = any(k.type_id in (LIST, STRUCT) for k in keys)
-    h = nested_hash("murmur", keys, seed) if nested else murmur_hash3_32(keys, seed)
+    h = nested_hash("murmur3", keys, seed) if nested else murmur_hash3_32(keys, seed)
     return spark_pmod(h.astype(np.int32), num_partitions)
 
 
