@@ -247,6 +247,43 @@ SRJ_API int srj_sha2_hash(int32_t digest_bits, const srj_column* input, const sr
  */
 SRJ_API int srj_host_crc32(uint32_t crc, const void* buf, int64_t len, uint32_t* out);
 
+/* ---- Spark BloomFilter: BloomFilter.create / put / merge / probe, bloom_filter.hpp:32-162, bloom_filter.cu:288-497 ------
+ * The serialized filter of Spark's BloomFilterImpl.writeTo, big-endian throughout:
+ *   V1: int32 {1, num_hashes, num_longs} (12 bytes), then num_longs longs
+ *   V2: int32 {2, num_hashes, seed, num_longs} (16 bytes), then num_longs longs
+ * Bit p lives in bit p % 64 of long p / 64; every position is taken modulo num_longs * 64.  A key x sets / tests the k
+ * positions of Spark's double hashing over h1 = Murmur3 hashLong(x, seed) and h2 = hashLong(x, h1) (seed 0 for V1): V1
+ * with 32-bit combined hashes, V2 with 64-bit ones (bloom_filter.cu:70-152).
+ *   srj_bloom_filter_sizes : (host only, no device) num_longs = ceil(bits / 64) and the serialized size.  SRJ_EINVAL for a
+ *                            version other than 1 / 2, num_hashes <= 0, bits <= 0, bits > INT32_MAX * 64 (the JNI shim
+ *                            throws IllegalArgumentException for these) or a size over INT32_MAX bytes.
+ *   srj_bloom_filter_init  : writes the header and zeroes the bit array of `filter` (the sizes call's total_bytes).
+ *   srj_bloom_filter_put   : sets the bits of every valid row of `input`; null rows are skipped.
+ *   srj_bloom_filter_probe : out[r] (BOOL8) = 1 when all the bits of row r are set.  The input mask is copied to out_mask
+ *                            when out_mask is not NULL (all valid when the input has none); an input with a mask needs
+ *                            out_mask.  Values under null rows are unspecified.  The output null count is the input's.
+ *   srj_bloom_filter_merge : `filters` holds num_filters serialized filters back to back (the child of a LIST<UINT8>
+ *                            column); `out` (filters_bytes / num_filters bytes) receives the first one's header and the
+ *                            word-wise OR of all bit arrays.  SRJ_EINVAL when the first header does not parse, when
+ *                            filters_bytes != num_filters x its size, or when any header differs from the first (version,
+ *                            num_hashes, seed or size).  The workspace holds srj_bloom_filter_merge_workspace_bytes() bytes.
+ * put / probe / merge read the filter's 16 header bytes back to the host once and synchronise the stream for it (the
+ * reference does the same in every call, bloom_filter.cu:201-203); merge reads its header-check flag back with that same
+ * synchronisation.  Errors of put / probe: a truncated filter, an unknown version, a bit array that is empty or whose size
+ * disagrees with filter_bytes, and (V1) num_longs * 64 > INT32_MAX are SRJ_EINVAL; an input that is not one INT64 column is
+ * SRJ_EUNSUPPORTED.  Filter and output buffers must be 4-byte aligned.
+ */
+#define SRJ_BLOOM_FILTER_VERSION_1 1
+#define SRJ_BLOOM_FILTER_VERSION_2 2
+SRJ_API int srj_bloom_filter_sizes(int32_t version, int32_t num_hashes, int64_t bits, int32_t* num_longs, int64_t* total_bytes);
+SRJ_API int srj_bloom_filter_init(int32_t version, int32_t num_hashes, int32_t num_longs, int32_t seed, uint8_t* filter, void* stream);
+SRJ_API int srj_bloom_filter_put(uint8_t* filter, int64_t filter_bytes, const srj_column* input, void* stream);
+SRJ_API int srj_bloom_filter_probe(const uint8_t* filter, int64_t filter_bytes, const srj_column* input, uint8_t* out,
+                                   uint32_t* out_mask, void* stream);
+SRJ_API int64_t srj_bloom_filter_merge_workspace_bytes(void);
+SRJ_API int srj_bloom_filter_merge(const uint8_t* filters, int64_t filters_bytes, int32_t num_filters, uint8_t* out, void* workspace,
+                                   void* stream);
+
 /* ---- multi-GPU configuration (SURVEY 8e: row-range shards + one all-gather of per-column chunks) ---------------- */
 /* ---- Spark HashPartitioning on the device (SURVEY 8f rank 1) ---------------------------------------------------
  * The consumer of Hash.murmurHash32: GpuHashPartitioning computes pmod(murmur3_32(42, keys), P) per row and then

@@ -1,0 +1,296 @@
+// bloom_filter.cu -- Spark's runtime-join bloom filter on the device (reference bloom_filter.cu, BloomFilter.java):
+// init, put, probe and merge of the serialized V1 / V2 formats.
+//
+// Format (bloom_filter.hpp:32-49, bloom_filter.cu:154-172): big-endian int32 header {1, k, numLongs} (12 B, V1) or
+// {2, k, seed, numLongs} (16 B, V2), then numLongs big-endian longs.  Bit p is bit p % 64 of long p / 64; in the
+// little-endian uint32 view of the bit array that is bit (p % 32) ^ 24 of word (p / 32) ^ 1 (bloom_filter.cu:60-66).
+// Every modulo is by bits = numLongs * 64.
+//
+// Element hashes (bloom_filter.cu:70-152, Spark's BloomFilterImpl / BloomFilterImplV2), all with Java int / long
+// wrap-around, done here in unsigned arithmetic:
+//   h1 = Murmur3_x86_32.hashLong(x, s), h2 = hashLong(x, h1); s = 0 (V1) or the header seed (V2)
+//   V1: for i = 1..k:  c = (int32)(h1 + i * h2),  p = (c < 0 ? ~c : c) % bits
+//   V2: c = (int64)h1 * INT32_MAX;  for i = 0..k-1:  c += (int64)h2,  p = (c < 0 ? ~c : c) % bits
+//
+// The modulo by the per-call constant `bits` uses a host-computed reciprocal m = floor((2^N - 1) / bits) (N = 32 for
+// V1's 31-bit dividends, 64 for V2's 63-bit ones): q = mulhi(x, m) is floor(x / bits) or one less (x < 2^(N-1) keeps
+// the error under 3/2), so r = x - q * bits needs at most one conditional subtraction.  No division instruction or
+// subroutine is left in the put / probe loops.
+#include "common.cuh"
+#include "hash_device.cuh"
+#include "kernels.hpp"
+
+namespace srj {
+namespace {
+
+constexpr int kBloomThreads = 256;
+constexpr int kRowsPerThread = 4;   // 2 x 16-byte key loads in, one 4-byte BOOL8 store out
+constexpr int kHashChunk     = 8;   // word loads of one row issued together before any is tested
+
+__device__ __forceinline__ uint32_t mod_v1(uint32_t x, uint32_t d, uint32_t m)
+{
+  uint32_t r = x - __umulhi(x, m) * d;
+  return r >= d ? r - d : r;
+}
+
+__device__ __forceinline__ uint64_t mod_v2(uint64_t x, uint64_t d, uint64_t m)
+{
+  uint64_t r = x - __umul64hi(x, m) * d;
+  return r >= d ? r - d : r;
+}
+
+// The k bit positions of one key, produced one at a time (V1 state in 32 bits, V2 in 64).
+template <int V>
+struct Positions {
+  uint64_t c, step;
+  __device__ __forceinline__ Positions(int64_t key, uint32_t seed)
+  {
+    const uint32_t h1 = hash::mm_u64(static_cast<uint64_t>(key), V == 1 ? 0u : seed);
+    const uint32_t h2 = hash::mm_u64(static_cast<uint64_t>(key), h1);
+    if (V == 1) {
+      c    = h1;
+      step = h2;
+    } else {
+      c    = static_cast<uint64_t>(static_cast<int64_t>(static_cast<int32_t>(h1)) * INT32_MAX);
+      step = static_cast<uint64_t>(static_cast<int64_t>(static_cast<int32_t>(h2)));
+    }
+  }
+  // next position (V1: i = 1, 2, ...; V2: i = 0, 1, ...; both start by adding h2)
+  __device__ __forceinline__ uint64_t next(uint64_t d, uint64_t m)
+  {
+    c += step;
+    if (V == 1) {
+      const uint32_t ci = static_cast<uint32_t>(c);
+      const uint32_t x  = ci ^ static_cast<uint32_t>(static_cast<int32_t>(ci) >> 31);   // c < 0 ? ~c : c
+      return mod_v1(x, static_cast<uint32_t>(d), static_cast<uint32_t>(m));
+    } else {
+      const uint64_t x = c ^ static_cast<uint64_t>(static_cast<int64_t>(c) >> 63);
+      return mod_v2(x, d, m);
+    }
+  }
+};
+
+__device__ __forceinline__ uint64_t word_of(uint64_t p) { return (p >> 5) ^ 1u; }
+__device__ __forceinline__ uint32_t bit_of(uint64_t p) { return 1u << ((static_cast<uint32_t>(p) & 31u) ^ 24u); }
+
+// the kRowsPerThread keys of this thread (rows [r0, r0 + count)); 16-byte loads when the keys are 16-byte aligned
+template <bool kVec>
+__device__ __forceinline__ void load_keys(const int64_t* __restrict__ keys, int64_t r0, int count, int64_t (&k)[kRowsPerThread])
+{
+  if (kVec && count == kRowsPerThread) {
+    const longlong2 a = __ldg(reinterpret_cast<const longlong2*>(keys + r0));
+    const longlong2 b = __ldg(reinterpret_cast<const longlong2*>(keys + r0 + 2));
+    k[0] = a.x; k[1] = a.y; k[2] = b.x; k[3] = b.y;
+  } else {
+#pragma unroll
+    for (int j = 0; j < kRowsPerThread; ++j) k[j] = j < count ? __ldg(keys + r0 + j) : 0;
+  }
+}
+
+// put: every valid row sets its k bits; atomicOr with the result unused compiles to RED.E.OR
+template <int V, bool kVec>
+__global__ void __launch_bounds__(kBloomThreads) bloom_put_kernel(uint32_t* __restrict__ words, uint64_t d, uint64_t m, int32_t k, uint32_t seed,
+                                                                  const int64_t* __restrict__ keys, const uint32_t* __restrict__ mask, int64_t n)
+{
+  const int64_t r0 = (static_cast<int64_t>(blockIdx.x) * kBloomThreads + threadIdx.x) * kRowsPerThread;
+  if (r0 >= n) return;
+  const int count = static_cast<int>(tmin<int64_t>(kRowsPerThread, n - r0));
+  int64_t key[kRowsPerThread];
+  load_keys<kVec>(keys, r0, count, key);
+  uint32_t valid = (1u << count) - 1u;                        // r0 is a multiple of 4: the rows share one mask word
+  if (mask) valid &= __ldg(mask + (r0 >> 5)) >> (r0 & 31);
+#pragma unroll
+  for (int j = 0; j < kRowsPerThread; ++j) {
+    if (!((valid >> j) & 1u)) continue;
+    Positions<V> pos(key[j], seed);
+    for (int32_t i = 0; i < k; ++i) {
+      const uint64_t p = pos.next(d, m);
+      atomicOr(words + word_of(p), bit_of(p));
+    }
+  }
+}
+
+// probe: out[r] = all k bits of row r are set.  Per chunk of kHashChunk hashes, the word loads of all the thread's rows
+// are issued (read-only path, L2-resident filter) before any is tested; a row whose chunk found a zero bit stops.
+// Rows under nulls are computed like the others (their values are not part of the result).
+template <int V, bool kVec>
+__global__ void __launch_bounds__(kBloomThreads) bloom_probe_kernel(const uint32_t* __restrict__ words, uint64_t d, uint64_t m, int32_t k, uint32_t seed,
+                                                                    const int64_t* __restrict__ keys, int64_t n, uint8_t* __restrict__ out)
+{
+  const int64_t r0 = (static_cast<int64_t>(blockIdx.x) * kBloomThreads + threadIdx.x) * kRowsPerThread;
+  if (r0 >= n) return;
+  const int count = static_cast<int>(tmin<int64_t>(kRowsPerThread, n - r0));
+  int64_t key[kRowsPerThread];
+  load_keys<kVec>(keys, r0, count, key);
+  Positions<V> pos[kRowsPerThread] = {Positions<V>(key[0], seed), Positions<V>(key[1], seed), Positions<V>(key[2], seed),
+                                      Positions<V>(key[3], seed)};
+  uint32_t hit = 0xfu;                                        // bit j: row j still has every bit seen so far set
+  for (int32_t i0 = 0; i0 < k && hit; i0 += kHashChunk) {
+    uint32_t w[kRowsPerThread][kHashChunk], b[kRowsPerThread][kHashChunk];
+#pragma unroll
+    for (int j = 0; j < kRowsPerThread; ++j)
+#pragma unroll
+      for (int i = 0; i < kHashChunk; ++i) {
+        b[j][i] = 0;
+        w[j][i] = 0;
+        if (i0 + i < k && ((hit >> j) & 1u)) {
+          const uint64_t p = pos[j].next(d, m);
+          b[j][i]          = bit_of(p);
+          w[j][i]          = __ldg(words + word_of(p));
+        }
+      }
+#pragma unroll
+    for (int j = 0; j < kRowsPerThread; ++j)
+#pragma unroll
+      for (int i = 0; i < kHashChunk; ++i)
+        if ((w[j][i] & b[j][i]) != b[j][i]) hit &= ~(1u << j);
+  }
+  uint32_t packed = 0;
+#pragma unroll
+  for (int j = 0; j < kRowsPerThread; ++j) packed |= ((hit >> j) & 1u) << (8 * j);
+  if (kVec && count == kRowsPerThread) {
+    *reinterpret_cast<uint32_t*>(out + r0) = packed;
+  } else {
+    for (int j = 0; j < count; ++j) out[r0 + j] = static_cast<uint8_t>((packed >> (8 * j)) & 1u);
+  }
+}
+
+// init: the big-endian header words, then zeros
+__global__ void __launch_bounds__(kBloomThreads) bloom_init_kernel(uint32_t* __restrict__ buf, int64_t nwords, uint4 hdr, int hdr_words)
+{
+  const int64_t stride = static_cast<int64_t>(gridDim.x) * kBloomThreads;
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * kBloomThreads + threadIdx.x; i < nwords; i += stride) {
+    uint32_t v = 0;
+    if (i < hdr_words) v = i == 0 ? hdr.x : i == 1 ? hdr.y : i == 2 ? hdr.z : hdr.w;
+    buf[i] = v;
+  }
+}
+
+// merge, header check: flag <- 1 when the header of any filter differs from the first one's
+__global__ void __launch_bounds__(kBloomThreads) bloom_merge_check_kernel(const uint32_t* __restrict__ child, int64_t stride_words, int32_t nfilters,
+                                                                          int hdr_words, int32_t* __restrict__ flag)
+{
+  const int64_t f = static_cast<int64_t>(blockIdx.x) * kBloomThreads + threadIdx.x + 1;
+  if (f >= nfilters) return;
+  bool same = true;
+  for (int i = 0; i < hdr_words; ++i) same &= __ldg(child + f * stride_words + i) == __ldg(child + i);
+  if (!same) *flag = 1;
+}
+
+// merge, bit arrays: dst[v] = OR over the filters of src_f[v], VW 32-bit words per access (16-byte accesses for VW = 4)
+template <int VW>
+struct Vec;
+template <> struct Vec<1> { using T = uint32_t; __device__ static T orv(T a, T b) { return a | b; } };
+template <> struct Vec<2> { using T = uint2; __device__ static T orv(T a, T b) { return make_uint2(a.x | b.x, a.y | b.y); } };
+template <> struct Vec<4> {
+  using T = uint4;
+  __device__ static T orv(T a, T b) { return make_uint4(a.x | b.x, a.y | b.y, a.z | b.z, a.w | b.w); }
+};
+
+template <int VW>
+__global__ void __launch_bounds__(kBloomThreads) bloom_merge_or_kernel(const uint8_t* __restrict__ src, int64_t stride_bytes, int32_t nfilters,
+                                                                       int64_t nvec, uint8_t* __restrict__ dst)
+{
+  using T        = typename Vec<VW>::T;
+  const int64_t v = static_cast<int64_t>(blockIdx.x) * kBloomThreads + threadIdx.x;
+  if (v >= nvec) return;
+  const T* s = reinterpret_cast<const T*>(src) + v;
+  const int64_t sv = stride_bytes / static_cast<int64_t>(sizeof(T));
+  T acc = __ldg(s);
+  int32_t f = 1;
+  for (; f + 4 <= nfilters; f += 4) {                          // four independent loads in flight per thread
+    const T a = __ldg(s + f * sv), b = __ldg(s + (f + 1) * sv), c = __ldg(s + (f + 2) * sv), e = __ldg(s + (f + 3) * sv);
+    acc = Vec<VW>::orv(acc, Vec<VW>::orv(Vec<VW>::orv(a, b), Vec<VW>::orv(c, e)));
+  }
+  for (; f < nfilters; ++f) acc = Vec<VW>::orv(acc, __ldg(s + f * sv));
+  reinterpret_cast<T*>(dst)[v] = acc;
+}
+
+unsigned grid_for(int64_t threads) { return static_cast<unsigned>((threads + kBloomThreads - 1) / kBloomThreads); }
+
+}  // namespace
+
+uint64_t bloom_reciprocal(int32_t version, uint64_t bits)
+{
+  return version == 1 ? static_cast<uint64_t>(0xffffffffu / static_cast<uint32_t>(bits)) : ~uint64_t{0} / bits;
+}
+
+int launch_bloom_init(const BloomHeader& h, uint8_t* buf, cudaStream_t stream)
+{
+  const int hdr_words = h.version == 1 ? 3 : 4;
+  auto bswap          = [](int32_t v) { return __builtin_bswap32(static_cast<uint32_t>(v)); };
+  const uint4 hdr     = h.version == 1 ? make_uint4(bswap(1), bswap(h.num_hashes), bswap(h.num_longs), 0u)
+                                       : make_uint4(bswap(2), bswap(h.num_hashes), bswap(h.seed), bswap(h.num_longs));
+  const int64_t nwords = hdr_words + 2 * static_cast<int64_t>(h.num_longs);
+  const unsigned grid  = static_cast<unsigned>(tmin<int64_t>(grid_for(nwords), 16 * sm_count()));
+  bloom_init_kernel<<<grid, kBloomThreads, 0, stream>>>(reinterpret_cast<uint32_t*>(buf), nwords, hdr, hdr_words);
+  SRJ_CUDA_TRY(cudaGetLastError());
+  return SRJ_OK;
+}
+
+int launch_bloom_put(const BloomHeader& h, uint8_t* buf, const srj_column& in, cudaStream_t stream)
+{
+  const int64_t n = in.size;
+  if (n == 0) return SRJ_OK;
+  auto* words       = reinterpret_cast<uint32_t*>(buf + (h.version == 1 ? 12 : 16));
+  const uint64_t d  = 64 * static_cast<uint64_t>(h.num_longs);
+  const uint64_t m  = bloom_reciprocal(h.version, d);
+  const auto* keys  = static_cast<const int64_t*>(in.data);
+  const bool vec    = (reinterpret_cast<uintptr_t>(keys) & 15) == 0;
+  const unsigned grid = grid_for((n + kRowsPerThread - 1) / kRowsPerThread);
+  const uint32_t seed = static_cast<uint32_t>(h.seed);
+#define SRJ_BLOOM_PUT(V, VEC) bloom_put_kernel<V, VEC><<<grid, kBloomThreads, 0, stream>>>(words, d, m, h.num_hashes, seed, keys, in.null_mask, n)
+  if (h.version == 1) { if (vec) SRJ_BLOOM_PUT(1, true); else SRJ_BLOOM_PUT(1, false); }
+  else                { if (vec) SRJ_BLOOM_PUT(2, true); else SRJ_BLOOM_PUT(2, false); }
+#undef SRJ_BLOOM_PUT
+  SRJ_CUDA_TRY(cudaGetLastError());
+  return SRJ_OK;
+}
+
+int launch_bloom_probe(const BloomHeader& h, const uint8_t* buf, const srj_column& in, uint8_t* out, uint32_t* out_mask, cudaStream_t stream)
+{
+  const int64_t n = in.size;
+  if (n == 0) return SRJ_OK;
+  if (out_mask) {
+    const size_t mask_bytes = static_cast<size_t>((n + 31) / 32) * 4;
+    if (in.null_mask) SRJ_CUDA_TRY(cudaMemcpyAsync(out_mask, in.null_mask, mask_bytes, cudaMemcpyDeviceToDevice, stream));
+    else SRJ_CUDA_TRY(cudaMemsetAsync(out_mask, 0xff, mask_bytes, stream));
+  }
+  const auto* words  = reinterpret_cast<const uint32_t*>(buf + (h.version == 1 ? 12 : 16));
+  const uint64_t d   = 64 * static_cast<uint64_t>(h.num_longs);
+  const uint64_t m   = bloom_reciprocal(h.version, d);
+  const auto* keys   = static_cast<const int64_t*>(in.data);
+  const bool vec     = (reinterpret_cast<uintptr_t>(keys) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 3) == 0;
+  const unsigned grid = grid_for((n + kRowsPerThread - 1) / kRowsPerThread);
+  const uint32_t seed = static_cast<uint32_t>(h.seed);
+#define SRJ_BLOOM_PROBE(V, VEC) bloom_probe_kernel<V, VEC><<<grid, kBloomThreads, 0, stream>>>(words, d, m, h.num_hashes, seed, keys, n, out)
+  if (h.version == 1) { if (vec) SRJ_BLOOM_PROBE(1, true); else SRJ_BLOOM_PROBE(1, false); }
+  else                { if (vec) SRJ_BLOOM_PROBE(2, true); else SRJ_BLOOM_PROBE(2, false); }
+#undef SRJ_BLOOM_PROBE
+  SRJ_CUDA_TRY(cudaGetLastError());
+  return SRJ_OK;
+}
+
+int launch_bloom_merge(const uint8_t* child, int64_t stride, int32_t nfilters, int hdr_bytes, uint8_t* out, int32_t* d_flag, cudaStream_t stream)
+{
+  SRJ_CUDA_TRY(cudaMemsetAsync(d_flag, 0, 4, stream));
+  if (nfilters > 1) {
+    bloom_merge_check_kernel<<<grid_for(nfilters - 1), kBloomThreads, 0, stream>>>(reinterpret_cast<const uint32_t*>(child), stride / 4, nfilters,
+                                                                                   hdr_bytes / 4, d_flag);
+    SRJ_CUDA_TRY(cudaGetLastError());
+  }
+  SRJ_CUDA_TRY(cudaMemcpyAsync(out, child, hdr_bytes, cudaMemcpyDeviceToDevice, stream));
+  const uint8_t* src    = child + hdr_bytes;
+  uint8_t* dst          = out + hdr_bytes;
+  const int64_t nbytes  = stride - hdr_bytes;
+  auto aligned = [&](int a) {
+    return (reinterpret_cast<uintptr_t>(src) % a) == 0 && (reinterpret_cast<uintptr_t>(dst) % a) == 0 && stride % a == 0 && nbytes % a == 0;
+  };
+  if (aligned(16)) bloom_merge_or_kernel<4><<<grid_for(nbytes / 16), kBloomThreads, 0, stream>>>(src, stride, nfilters, nbytes / 16, dst);
+  else if (aligned(8)) bloom_merge_or_kernel<2><<<grid_for(nbytes / 8), kBloomThreads, 0, stream>>>(src, stride, nfilters, nbytes / 8, dst);
+  else bloom_merge_or_kernel<1><<<grid_for(nbytes / 4), kBloomThreads, 0, stream>>>(src, stride, nfilters, nbytes / 4, dst);
+  SRJ_CUDA_TRY(cudaGetLastError());
+  return SRJ_OK;
+}
+
+}  // namespace srj

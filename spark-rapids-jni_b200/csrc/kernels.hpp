@@ -107,6 +107,18 @@ int64_t sha2_workspace_bytes(int64_t n);
 int launch_sha2_sizes(int32_t digest_bits, const srj_column& in, int32_t* d_offsets, int64_t* h_total, void* workspace, cudaStream_t stream);
 int launch_sha2(int32_t digest_bits, const srj_column& in, const srj_column& out, cudaStream_t stream);
 
+// ---- bloom_filter.cu: Spark's serialized V1 / V2 bloom filter (init, put, probe, merge) ----
+struct BloomHeader {
+  int32_t version, num_hashes, seed, num_longs;   // seed is 0 for V1
+};
+// m with x % bits == x - mulhi(x, m) * bits, minus bits once more when that is >= bits (32-bit x for V1, 64-bit for V2)
+uint64_t bloom_reciprocal(int32_t version, uint64_t bits);
+int launch_bloom_init(const BloomHeader& h, uint8_t* buf, cudaStream_t stream);
+int launch_bloom_put(const BloomHeader& h, uint8_t* buf, const srj_column& in, cudaStream_t stream);
+int launch_bloom_probe(const BloomHeader& h, const uint8_t* buf, const srj_column& in, uint8_t* out, uint32_t* out_mask, cudaStream_t stream);
+// header copy, header check (*d_flag <- 1 on a mismatch) and the word-wise OR of `nfilters` filters `stride` bytes apart
+int launch_bloom_merge(const uint8_t* child, int64_t stride, int32_t nfilters, int hdr_bytes, uint8_t* out, int32_t* d_flag, cudaStream_t stream);
+
 // ---- kudo.cu: the Kudo shuffle wire format for flat tables (split / assemble) ----
 int64_t kudo_workspace_bytes(int32_t ncols, int32_t P);
 int launch_kudo_split_sizes(const srj_column* cols, int32_t ncols, const int32_t* d_splits, int32_t P, int64_t* d_part_offsets, int64_t* h_total,

@@ -4,28 +4,11 @@
 // from any translation unit of the loaded library.
 // Input: one cudf::column_view* of type STRING; output: a heap cudf::column* STRING of lowercase hex digests with the
 // input's null mask and null count.
-#include <exception>
-#include <new>
-
 #include "srj_jni_common.hpp"
 
 using namespace srjshim;
 
 namespace {
-
-// No C++ exception (rmm::out_of_memory, std::bad_alloc, ...) may leave a JNI function: map them to the Java classes.
-void throw_from_exception(JNIEnv* env)
-{
-  try {
-    throw;
-  } catch (const std::bad_alloc& e) {
-    throw_java(env, "java/lang/OutOfMemoryError", e.what());
-  } catch (const std::exception& e) {
-    throw_java(env, "ai/rapids/cudf/CudfException", e.what());
-  } catch (...) {
-    throw_java(env, "ai/rapids/cudf/CudfException", "unknown C++ exception");
-  }
-}
 
 jlong sha2_nulls_preserved(JNIEnv* env, int32_t digest_bits, jlong column_handle)
 {

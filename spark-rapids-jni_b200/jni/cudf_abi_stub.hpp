@@ -2,7 +2,7 @@
 // syntax-checked without libcudf (this image has neither libcudf nor rmm headers).  Field meanings follow
 // thirdparty/cudf/cpp/include/cudf/column/column_view.hpp:237-244 and types.hpp:191-224; a real build includes
 // <cudf/column/column_view.hpp>, <cudf/table/table_view.hpp>, <cudf/column/column_factories.hpp>,
-// <cudf/lists/lists_column_view.hpp>, <rmm/device_buffer.hpp>, <rmm/cuda_stream_view.hpp> instead.
+// <cudf/lists/lists_column_view.hpp>, <cudf/scalar/scalar.hpp>, <rmm/device_buffer.hpp>, <rmm/cuda_stream_view.hpp> instead.
 #pragma once
 #include <cstddef>
 #include <cstdint>
@@ -22,7 +22,7 @@ struct device_buffer {
 namespace cudf {
 using size_type     = int32_t;
 using bitmask_type  = uint32_t;
-enum class type_id : int32_t { EMPTY = 0, INT8 = 1, UINT8 = 5, INT32 = 3, INT64 = 4, STRING = 23, LIST = 24 };
+enum class type_id : int32_t { EMPTY = 0, INT8 = 1, UINT8 = 5, INT32 = 3, INT64 = 4, BOOL8 = 11, STRING = 23, LIST = 24 };
 struct data_type {
   data_type(type_id id, int32_t scale = 0);
   type_id id() const;
@@ -53,6 +53,15 @@ struct column {
   column(data_type type, size_type size, rmm::device_buffer&& data, rmm::device_buffer&& null_mask, size_type null_count);
   mutable_column_view mutable_view();
   void set_null_count(size_type n);
+};
+struct lists_column_view {                           // lists/lists_column_view.hpp
+  explicit lists_column_view(column_view const& lists);
+  column_view child() const;
+  size_type size() const;
+};
+struct list_scalar {                                 // scalar/scalar.hpp: one row of a LIST column, held by its child
+  list_scalar(column&& data, bool is_valid, rmm::cuda_stream_view stream);
+  column_view view() const;
 };
 std::unique_ptr<column> make_lists_column(size_type num_rows, std::unique_ptr<column> offsets, std::unique_ptr<column> child,
                                           size_type null_count, rmm::device_buffer&& null_mask);

@@ -15,8 +15,10 @@
 #include "cudf_jni_apis.hpp"
 #endif
 
+#include <exception>
 #include <map>
 #include <mutex>
+#include <new>
 #include <string>
 #include <utility>
 #include <vector>
@@ -41,6 +43,21 @@ inline bool throw_if_error(JNIEnv* env, int status)
 inline void throw_java(JNIEnv* env, const char* cls, const char* msg)
 {
   if (!env->ExceptionCheck()) env->ThrowNew(env->FindClass(cls), msg);
+}
+
+// No C++ exception (rmm::out_of_memory, std::bad_alloc, ...) may leave a JNI function: map them to the Java classes.
+// Call from a catch (...) block.
+inline void throw_from_exception(JNIEnv* env)
+{
+  try {
+    throw;
+  } catch (const std::bad_alloc& e) {
+    throw_java(env, "java/lang/OutOfMemoryError", e.what());
+  } catch (const std::exception& e) {
+    throw_java(env, "ai/rapids/cudf/CudfException", e.what());
+  } catch (...) {
+    throw_java(env, "ai/rapids/cudf/CudfException", "unknown C++ exception");
+  }
 }
 
 // One srj_plan per (device, schema): plans are immutable and thread-safe, so concurrent Spark tasks share them.
