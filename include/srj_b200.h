@@ -325,7 +325,8 @@ SRJ_API int srj_partition_strings(const srj_column* in, const srj_column* out, i
  * kudo/KudoSerializer.java:49-171 (header "KUD0" + 6 big-endian ints + hasValidity bits | validity | offsets | data);
  * assemble concatenates partitions (of one or several splits) back into one table.
  *   srj_kudo_split_sizes    : d_partition_offsets[P + 1] (byte offset of every partition) and *total_bytes (host; one
- *                             stream synchronisation).
+ *                             stream synchronisation).  SRJ_EINVAL when a split lies outside [0, num_rows],
+ *                             SRJ_EOVERFLOW when the splits decrease or a partition overflows the header's lengths.
  *   srj_kudo_split          : writes the partitions into `out` (total_bytes, 4-byte aligned).
  *   srj_kudo_assemble_sizes : parses the headers; *total_rows and, per STRING column, char_totals[c] (host arrays);
  *                             SRJ_EINVAL on a malformed header.  The workspace keeps what srj_kudo_assemble needs.

@@ -914,6 +914,9 @@ int srj_hash_partition(const srj_column* keys, int32_t num_keys, int64_t num_row
   SRJ_API_RANGE();
   if (num_keys <= 0 || !keys) { set_error("hash_partition: no key columns"); return SRJ_EINVAL; }
   if (num_rows > 0 && !d_partition_ids) { set_error("hash_partition: bad argument"); return SRJ_EINVAL; }
+  // the partition count is checked before the keys are hashed: a refused call launches nothing
+  if (num_partitions <= 0) { set_error("hash_partition: %d partitions", num_partitions); return SRJ_EINVAL; }
+  if (num_partitions > (1 << 14)) { set_error("hash_partition: %d partitions exceed 16384 partitions", num_partitions); return SRJ_EUNSUPPORTED; }
   // the hashes go where the ids will be: part_ids_kernel turns them into ids in place
   int rc = hash_any(SRJ_HASH_MURMUR3_32, keys, num_keys, num_rows, seed, d_partition_ids, static_cast<cudaStream_t>(stream));
   if (rc != SRJ_OK) return rc;
@@ -1082,8 +1085,10 @@ int srj_kudo_split_sizes(const srj_column* cols, int32_t num_columns, int64_t nu
   if (!d_splits || !total_bytes || num_rows < 0 || num_rows > INT32_MAX) { set_error("kudo_split_sizes: bad argument"); return SRJ_EINVAL; }
   for (int32_t c = 0; c < num_columns; ++c)
     if (cols[c].size != num_rows) { set_error("kudo_split_sizes: column %d: row count mismatch", c); return SRJ_EINVAL; }
-  rc = launch_kudo_split_sizes(cols, num_columns, d_splits, num_partitions, d_partition_offsets, total_bytes, workspace, static_cast<cudaStream_t>(stream));
+  rc = launch_kudo_split_sizes(cols, num_columns, num_rows, d_splits, num_partitions, d_partition_offsets, total_bytes, workspace,
+                               static_cast<cudaStream_t>(stream));
   if (rc == SRJ_EUNSUPPORTED) set_error("kudo_split_sizes: only fixed-width, decimal and STRING columns");
+  else if (rc == SRJ_EINVAL) set_error("kudo_split_sizes: the splits must lie in [0, %lld]", static_cast<long long>(num_rows));
   else if (rc == SRJ_EOVERFLOW) set_error("kudo_split_sizes: a partition exceeds the 32-bit section lengths of the Kudo header, or the splits are not increasing");
   return rc;
 }

@@ -121,8 +121,8 @@ int launch_bloom_merge(const uint8_t* child, int64_t stride, int32_t nfilters, i
 
 // ---- kudo.cu: the Kudo shuffle wire format for flat tables (split / assemble) ----
 int64_t kudo_workspace_bytes(int32_t ncols, int32_t P);
-int launch_kudo_split_sizes(const srj_column* cols, int32_t ncols, const int32_t* d_splits, int32_t P, int64_t* d_part_offsets, int64_t* h_total,
-                            void* workspace, cudaStream_t stream);
+int launch_kudo_split_sizes(const srj_column* cols, int32_t ncols, int64_t num_rows, const int32_t* d_splits, int32_t P, int64_t* d_part_offsets,
+                            int64_t* h_total, void* workspace, cudaStream_t stream);
 int launch_kudo_split(const srj_column* cols, int32_t ncols, const int32_t* d_splits, int32_t P, const int64_t* d_part_offsets, uint8_t* out,
                       void* workspace, cudaStream_t stream);
 int launch_kudo_assemble_sizes(const uint8_t* buf, const int64_t* d_part_offsets, int32_t P, const int32_t* type_ids, int32_t ncols, int64_t* h_rows,

@@ -82,12 +82,19 @@ __device__ void cta_copy_bytes(uint8_t* __restrict__ dst, const uint8_t* __restr
 }
 
 // ---- split ---------------------------------------------------------------------------------------------------------------
+// *bad: bit 0 = a partition too large for the header, or splits not increasing; bit 1 = a split outside [0, num_rows]
 __global__ void __launch_bounds__(256) kudo_split_sizes_kernel(const KCol* __restrict__ cols, int ncols, const int32_t* __restrict__ splits, int P,
-                                                              int64_t* __restrict__ part_sizes, int32_t* __restrict__ bad)
+                                                              int64_t num_rows, int64_t* __restrict__ part_sizes, int32_t* __restrict__ bad)
 {
   const int p = blockIdx.x * 256 + threadIdx.x;
   if (p >= P) return;
   const int32_t s = splits[p], n = splits[p + 1] - s;
+  // checked before any column is read: the STRING sizes read offsets[s] and offsets[s + n]
+  if (s < 0 || splits[p + 1] > num_rows || n < 0) {
+    part_sizes[p] = 0;
+    atomicOr(bad, n < 0 ? 1 : 2);
+    return;
+  }
   int64_t V = 0, O = 0, D = 0;
   for (int c = 0; c < ncols; ++c) {
     int64_t v, o, d;
@@ -99,7 +106,7 @@ __global__ void __launch_bounds__(256) kudo_split_sizes_kernel(const KCol* __res
   const int hs  = kudo_header_bytes(ncols);
   part_sizes[p] = pad4(hs + V) + pad4(O) + pad4(D);
   // the header holds the section lengths as 32-bit integers (KudoTableHeaderCalc.java:70-77: toIntExact)
-  if (n < 0 || pad4(hs + V) - hs + pad4(O) + pad4(D) > INT32_MAX) atomicExch(bad, 1);
+  if (pad4(hs + V) - hs + pad4(O) + pad4(D) > INT32_MAX) atomicOr(bad, 1);
 }
 
 // exclusive scan of P + 1 int64 in place by one CTA (P <= a few 10^4); element P receives the total
@@ -387,22 +394,22 @@ static int kudo_upload(const srj_column* cols, int32_t ncols, const KudoWs& ws, 
   return SRJ_OK;
 }
 
-int launch_kudo_split_sizes(const srj_column* cols, int32_t ncols, const int32_t* d_splits, int32_t P, int64_t* d_part_offsets, int64_t* h_total,
-                            void* workspace, cudaStream_t stream)
+int launch_kudo_split_sizes(const srj_column* cols, int32_t ncols, int64_t num_rows, const int32_t* d_splits, int32_t P, int64_t* d_part_offsets,
+                            int64_t* h_total, void* workspace, cudaStream_t stream)
 {
   const KudoWs ws = kudo_ws(workspace, P);
   int nstr = 0;
   const int rc = kudo_upload(cols, ncols, ws, &nstr, stream);
   if (rc != SRJ_OK) return rc;
   SRJ_CUDA_TRY(cudaMemsetAsync(ws.bad, 0, 4, stream));
-  kudo_split_sizes_kernel<<<(P + 255) / 256, 256, 0, stream>>>(ws.cols, ncols, d_splits, P, d_part_offsets, ws.bad);
+  kudo_split_sizes_kernel<<<(P + 255) / 256, 256, 0, stream>>>(ws.cols, ncols, d_splits, P, num_rows, d_part_offsets, ws.bad);
   i64_scan_small_kernel<<<1, 1024, 0, stream>>>(d_part_offsets, P);
   SRJ_CUDA_TRY(cudaGetLastError());
   int32_t bad = 0;
   SRJ_CUDA_TRY(cudaMemcpyAsync(h_total, d_part_offsets + P, 8, cudaMemcpyDeviceToHost, stream));
   SRJ_CUDA_TRY(cudaMemcpyAsync(&bad, ws.bad, 4, cudaMemcpyDeviceToHost, stream));
   SRJ_CUDA_TRY(cudaStreamSynchronize(stream));
-  return bad ? SRJ_EOVERFLOW : SRJ_OK;
+  return (bad & 2) ? SRJ_EINVAL : bad ? SRJ_EOVERFLOW : SRJ_OK;
 }
 
 int launch_kudo_split(const srj_column* cols, int32_t ncols, const int32_t* d_splits, int32_t P, const int64_t* d_part_offsets, uint8_t* out,
