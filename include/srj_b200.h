@@ -167,8 +167,8 @@ SRJ_API int srj_convert_to_rows(const srj_plan* plan, const srj_column* cols, in
  *                 its fast path.  Bit 1 set = a STRING column's chars exceed INT32_MAX (the caller maps it to
  *                 SRJ_EOVERFLOW / CudfColumnSizeOverflowException; the totals themselves are exact int64).
  *                 The STRING offsets children are complete only after phase 2.
- * If hash_kind != SRJ_HASH_NONE the row hash of the listed key columns is computed from the same
- * shared-memory tile and written to hash_out (int64 for xxhash64, int32 otherwise): the fused
+ * If hash_kind != SRJ_HASH_NONE the row hash of the listed key columns is computed in the same call, from
+ * the key columns just written, and written to hash_out (int64 for xxhash64, int32 otherwise): the fused
  * from_rows + partition-hash of BASELINE config 4.  Keys must be fixed-width columns.
  */
 /*

@@ -21,8 +21,6 @@ FLAGS = [
     "--shared", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "-ccbin", "/usr/bin/g++",
     "--expt-relaxed-constexpr", "-Xptxas", "-v" if os.environ.get("SRJ_PTXAS_V") else "-O3",
 ]
-if os.environ.get("SRJ_DEV_KNOBS"):      # development builds only: tuning knobs read from the environment (common.cuh)
-    FLAGS.append("-DSRJ_DEV_KNOBS")
 
 
 def needs_build() -> bool:

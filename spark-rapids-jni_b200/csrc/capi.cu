@@ -145,10 +145,10 @@ struct TableLease {
   }
 };
 
-// Phase 1 of a wide variable-width table runs from_rows_wide_kernel (no fused hash there).
-static bool use_wide_from_rows(const srj_plan* plan, const int32_t* row_offsets, const srj_fused_hash* hash)
+// Phase 1 of a wide variable-width table runs from_rows_wide_kernel.
+static bool use_wide_from_rows(const srj_plan* plan, const int32_t* row_offsets)
 {
-  return plan->wide.enabled && row_offsets != nullptr && !(hash && hash->kind != SRJ_HASH_NONE);
+  return plan->wide.enabled && row_offsets != nullptr;
 }
 
 static int check_cols(const srj_plan* plan, const srj_column* cols, int64_t num_rows, const char* who)
@@ -249,10 +249,6 @@ int srj_plan_create(const int32_t* type_ids, const int32_t* scales, int32_t num_
   if (R > 512) R = 512;
   if (R >= 128) R = R / 128 * 128;  // 4 row groups per unit => predicate-free fast path
   if (R < 32) R = fitrows >= 16 ? 16 : 8;
-  // development knobs (tuning only)
-  if (const int v = SRJ_KNOB("SRJ_FR_STAGES", 0)) tl.num_stages = v;
-  if (const int v = SRJ_KNOB("SRJ_FR_TILE_ROWS", 0)) { R = v; tl.stage_bytes = std::max(R * S, 4096); }
-  if (const int v = SRJ_KNOB("SRJ_FR_STAGE_KB", 0)) tl.stage_bytes = v * 1024;
   tl.tile_rows     = R;
   tl.rows_per_item = R >= 32 ? 32 : R;
   // The per-schema shared-memory tables (entry starts, column and mask pointers, null counters) come on top of the
@@ -527,25 +523,20 @@ int srj_convert_from_rows_fixed(const srj_plan* plan, const uint8_t* rows, const
     }
     if (!cols[c].null_mask && num_rows > 0) { set_error("convert_from_rows: column %d has no null mask buffer (always allocated, RC:2220)", c); return SRJ_EINVAL; }
   }
-  // The hash of a "fused" call can run inside the conversion kernel (no extra traffic: the consumer warps hash the key
-  // fields they already hold) or as the streaming hash kernel over the key columns just written (12 more bytes per row
-  // for two integer keys, but the conversion kernel keeps its issue slots for the transpose and the hash its own kernel
-  // shape).  SRJ_FUSE_SPLIT picks the second; it also lets wide variable-width tables keep their fast path.
-  const bool want_hash  = hash && hash->kind != SRJ_HASH_NONE;
-  const bool split_hash = want_hash && SRJ_KNOB("SRJ_FUSE_SPLIT", 1) != 0;
-  const srj_fused_hash* fused = split_hash ? nullptr : hash;
+  // The hash of a "fused" call is the streaming hash kernel over the key columns just written (12 more bytes per row
+  // for two integer keys, but the conversion kernel keeps its issue slots for the transpose and the hash its own
+  // kernel shape), so wide variable-width tables keep their fast path too.
   auto hash_after = [&]() -> int {
-    if (!split_hash || num_rows == 0) return SRJ_OK;
+    if (!hash || hash->kind == SRJ_HASH_NONE || num_rows == 0) return SRJ_OK;
     srj_column keys[16];
     for (int k = 0; k < hash->num_keys; ++k) keys[k] = cols[hash->key_columns[k]];
     return launch_hash(hash->kind, keys, hash->num_keys, num_rows, hash->seed, hash->out, stream);
   };
-  if (use_wide_from_rows(plan, row_offsets, fused)) {
+  if (use_wide_from_rows(plan, row_offsets)) {
     // wide variable-width table: per-row slabs; the pointer tables travel as kernel parameters and the kernels publish
     // null counts / totals / status themselves: no memset, no staging copy, no hidden allocation
     if (num_rows > 0 && !workspace) { set_error("convert_from_rows: this schema needs a workspace (srj_from_rows_workspace_bytes)"); return SRJ_EINVAL; }
-    rc = launch_from_rows_wide(plan, rows, row_offsets, rows_bytes, num_rows, cols, d_null_counts, d_char_totals, workspace,
-                               SRJ_KNOB("SRJ_W_FINALIZE", 0) != 0, stream);
+    rc = launch_from_rows_wide(plan, rows, row_offsets, rows_bytes, num_rows, cols, d_null_counts, d_char_totals, workspace, stream);
     return rc != SRJ_OK ? rc : hash_after();
   }
   if (d_null_counts) SRJ_CUDA_TRY(cudaMemsetAsync(d_null_counts, 0, sizeof(int64_t) * nc, stream));
@@ -570,12 +561,12 @@ int srj_convert_from_rows_fixed(const srj_plan* plan, const uint8_t* rows, const
   if (rc != SRJ_OK) return rc;
   auto** d = static_cast<void**>(sc.dev());
   rc = launch_from_rows(plan, rows, row_offsets, rows_bytes, num_rows, d, reinterpret_cast<uint32_t* const*>(d + nent),
-                        d_null_counts, d_char_totals ? d_char_totals + nc : nullptr, fused, stream);
+                        d_null_counts, d_char_totals ? d_char_totals + nc : nullptr, stream);
   if (rc != SRJ_OK) return rc;
   if (nstr > 0) {
     uint8_t* tail = static_cast<uint8_t*>(sc.dev()) + tab_bytes;
     rc = launch_string_offsets_scan(reinterpret_cast<int32_t* const*>(d + nent + nc), plan->d_string_cols, nstr, num_rows,
-                                    d_char_totals, d_char_totals ? d_char_totals + nc : nullptr, tail, plan->wide.enabled, stream);
+                                    d_char_totals, d_char_totals ? d_char_totals + nc : nullptr, tail, stream);
     if (rc != SRJ_OK) return rc;
   }
   return hash_after();
@@ -597,7 +588,7 @@ int srj_convert_from_rows_strings(const srj_plan* plan, const uint8_t* rows, con
   const int64_t* d_status = d_char_totals ? d_char_totals + plan->num_columns : nullptr;
   // wide tables: phase 1 (from_rows_wide.cu) left group-local offsets + the group bases in the workspace
   const uint32_t* d_bases = nullptr;
-  if (plan->wide.enabled && SRJ_KNOB("SRJ_W_FINALIZE", 0) == 0) {
+  if (plan->wide.enabled) {
     if (!workspace) { set_error("convert_from_rows_strings: this schema needs the workspace phase 1 filled"); return SRJ_EINVAL; }
     d_bases = wide_workspace_bases(plan, num_rows, workspace);
   }

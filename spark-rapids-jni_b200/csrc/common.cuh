@@ -20,16 +20,6 @@ int sm_count();  // multiprocessors of the current device (grid caps of the grid
     if (_e != cudaSuccess) return ::srj::cuda_fail(_e, #expr); \
   } while (0)
 
-// ---- development knobs ------------------------------------------------------------------------------
-// Tuning knobs read from the environment exist only in development builds (-DSRJ_DEV_KNOBS, see build.py); a
-// release build compiles every SRJ_KNOB to its default.  Each site reads its variable once.
-#ifdef SRJ_DEV_KNOBS
-#include <cstdlib>
-#define SRJ_KNOB(name, dflt) ([]() -> int { static const int v = []() { const char* e = getenv(name); return e ? atoi(e) : (dflt); }(); return v; }())
-#else
-#define SRJ_KNOB(name, dflt) (dflt)
-#endif
-
 // ---- device: shared-memory address + mbarrier + bulk copies -----------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p)
 {

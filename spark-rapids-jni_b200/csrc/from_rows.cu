@@ -1,7 +1,7 @@
 // from_rows.cu -- JCUDF rows -> columns (reference: convert_from_rows, RC:2149-2441).
 //
 // One persistent, warp-specialised kernel replaces copy_from_rows + copy_validity_from_rows +
-// fixup_null_counts (RC:879-969, 987-1094, 2130-2136) and optionally fuses the partition hash:
+// fixup_null_counts (RC:879-969, 987-1094, 2130-2136):
 //
 //   producer warp : walks the CTA's contiguous row range tile by tile; each tile is ONE contiguous
 //                   byte range of the row buffer, moved global->shared by a single 1-D TMA bulk copy
@@ -10,8 +10,7 @@
 //   consumer warps: lane = row.  A work unit is (field, chunk of row groups): a few shared-memory
 //                   reads of one field of 32 consecutive rows, batched for ILP, then coalesced
 //                   st.global stores into the column; validity bytes are bit-transposed with
-//                   __ballot_sync into the column masks; null counts are popc'd on the way; the row
-//                   hash of the key columns is computed in registers from the same tile.
+//                   __ballot_sync into the column masks; null counts are popc'd on the way.
 //
 // The unit -> (field, chunk) map is a shift/mask of host-computed constants; full tiles of
 // fixed-stride tables run a predicate-free instantiation.  Rows whose tile cannot be staged (row
@@ -22,7 +21,6 @@
 #include <vector>
 
 #include "common.cuh"
-#include "hash_device.cuh"
 #include "kernels.hpp"
 #include "movers.cuh"
 #include "plan.hpp"
@@ -71,14 +69,6 @@ struct FromRowsParams {
   int32_t size_per_row;
   const int32_t* string_start;   // [nstr] row byte offset of each (offset, len) pair
   unsigned long long* status;    // bit 0 <- 1 when a row's pair.offset differs from the canonical position
-  // fused hash
-  int32_t hash_kind;
-  int32_t hash_nkeys;
-  int32_t key_start[16];
-  int32_t key_type[16];
-  int32_t key_col[16];
-  int64_t hash_seed;
-  void* hash_out;
 };
 
 template <bool SAFE>
@@ -101,44 +91,6 @@ __device__ __forceinline__ uint64_t load_key(const uint8_t* p, int sz)
   }
 }
 
-// 4 / 8: the key is hashed as the 4- / 8-byte value stored in the row (xxhash64.cu / murmur_hash.cuh element
-// hashers for 32- and 64-bit integers, dates, timestamps, durations, DECIMAL64); 0: needs widening or normalising
-__device__ __forceinline__ int plain_key_bytes(int32_t t)
-{
-  switch (t) {
-    case SRJ_INT32: case SRJ_UINT32: case SRJ_TIMESTAMP_DAYS: case SRJ_DURATION_DAYS: return 4;
-    case SRJ_INT64: case SRJ_UINT64: case SRJ_TIMESTAMP_SECONDS: case SRJ_TIMESTAMP_MILLISECONDS:
-    case SRJ_TIMESTAMP_MICROSECONDS: case SRJ_TIMESTAMP_NANOSECONDS: case SRJ_DURATION_SECONDS:
-    case SRJ_DURATION_MILLISECONDS: case SRJ_DURATION_MICROSECONDS: case SRJ_DURATION_NANOSECONDS:
-    case SRJ_DECIMAL64: return 8;
-    default: return 0;
-  }
-}
-
-__device__ __forceinline__ int key_size(int32_t t)
-{
-  switch (t) {
-    case SRJ_INT8: case SRJ_UINT8: case SRJ_BOOL8: return 1;
-    case SRJ_INT16: case SRJ_UINT16: return 2;
-    case SRJ_INT32: case SRJ_UINT32: case SRJ_FLOAT32: case SRJ_TIMESTAMP_DAYS: case SRJ_DURATION_DAYS:
-    case SRJ_DECIMAL32: return 4;
-    case SRJ_DECIMAL128: return 16;
-    default: return 8;
-  }
-}
-
-// Fused-hash parameters, copied to shared memory once per CTA: the out-of-line hash code must not reach
-// into the kernel parameter struct through a generic pointer (each access becomes a global-path load).
-struct HashSpec {
-  int32_t kind, nkeys, validity_offset;
-  int32_t plain;  // 1: every key is a 4- or 8-byte integer-like value (hashed as is): two-chains path
-  int32_t key_start[16];
-  int32_t key_type[16];
-  int32_t key_col[16];
-  int64_t seed;
-  void* out;
-};
-
 // Shared-memory resident copies of the schedule (filled once per CTA).
 struct SmemTables {
   const int32_t* ent_start;  // [nentries]
@@ -146,7 +98,6 @@ struct SmemTables {
   uint32_t* const* masks;    // [ncols]
   int32_t* nulls;            // [ncols] or NULL
   const int32_t* string_start;  // [nstr]
-  const HashSpec* hash;         // NULL when no hash is fused
 };
 
 // Per-consumer-warp schedule constants, computed once per CTA.
@@ -324,99 +275,6 @@ __device__ __forceinline__ void validity_tile(const FromRowsParams& p, const Sme
   }
 }
 
-// ---- fused row hash of the key columns (lane = row), chained across keys with the Spark rules ------------
-template <int NCW, bool VAR, bool SAFE>
-__device__ __noinline__ void hash_tile(const HashSpec* hs, const uint8_t* base, const int32_t* s_off, uint32_t stride,
-                                       int64_t r0, int rows, int cw)
-{
-  TileView tv;
-  tv.base   = base;
-  tv.s_off  = s_off;
-  tv.stride = stride;
-  const int lane  = lane_id();
-  const int ng32  = (rows + 31) >> 5;
-  const int kind  = hs->kind;
-  const int nkeys = hs->nkeys;
-  const int voff  = hs->validity_offset;
-  // The hash of a row is one long dependent multiply chain, so a 32-row group is slow on its warp.  The
-  // groups are dealt to the warps starting at a different warp every tile: consumers only meet at the
-  // stage barriers (up to two tiles apart), so the extra group a warp gets on one tile is absorbed.
-  const int rot = static_cast<int>((r0 / tmax(rows, 1)) % NCW);
-  if (!SAFE && hs->plain) {
-    // Plain keys: a warp hashes TWO of its row groups at once -- two independent multiply chains per lane --
-    // (the element hash is a serial dependency chain; one chain per warp leaves the integer pipe idle).
-    const bool xx = kind == SRJ_HASH_XXHASH64;
-    for (int g = (cw + NCW - rot) % NCW; g < ng32; g += 2 * NCW) {
-      const int rowA = g * 32 + lane, rowB = rowA + NCW * 32;
-      const bool inA = rowA < rows, inB = rowB < rows;
-      const uint8_t* rpA = row_ptr<VAR>(tv, inA ? rowA : 0);
-      const uint8_t* rpB = row_ptr<VAR>(tv, inB ? rowB : 0);
-      uint64_t hA = static_cast<uint64_t>(hs->seed), hB = hA;
-      for (int k = 0; k < nkeys; ++k) {
-        const int c       = hs->key_col[k];
-        const int st      = hs->key_start[k];
-        const bool four   = plain_key_bytes(hs->key_type[k]) == 4;
-        const bool validA = (rpA[voff + (c >> 3)] >> (c & 7)) & 1u;
-        const bool validB = (rpB[voff + (c >> 3)] >> (c & 7)) & 1u;
-        uint64_t tA, tB;
-        if (four) {
-          const uint32_t vA = *reinterpret_cast<const uint32_t*>(rpA + st);
-          const uint32_t vB = *reinterpret_cast<const uint32_t*>(rpB + st);
-          if (xx) { tA = hash::xx_u32(vA, hA); tB = hash::xx_u32(vB, hB); }
-          else { tA = hash::mm_u32(vA, static_cast<uint32_t>(hA)); tB = hash::mm_u32(vB, static_cast<uint32_t>(hB)); }
-        } else {
-          const uint64_t vA = load_key<false>(rpA + st, 8);
-          const uint64_t vB = load_key<false>(rpB + st, 8);
-          if (xx) { tA = hash::xx_u64(vA, hA); tB = hash::xx_u64(vB, hB); }
-          else { tA = hash::mm_u64(vA, static_cast<uint32_t>(hA)); tB = hash::mm_u64(vB, static_cast<uint32_t>(hB)); }
-        }
-        hA = validA ? tA : hA;  // a null keeps the accumulator (Spark)
-        hB = validB ? tB : hB;
-      }
-      if (xx) {
-        if (inA) reinterpret_cast<uint64_t*>(hs->out)[r0 + rowA] = hA;
-        if (inB) reinterpret_cast<uint64_t*>(hs->out)[r0 + rowB] = hB;
-      } else {
-        if (inA) reinterpret_cast<uint32_t*>(hs->out)[r0 + rowA] = static_cast<uint32_t>(hA);
-        if (inB) reinterpret_cast<uint32_t*>(hs->out)[r0 + rowB] = static_cast<uint32_t>(hB);
-      }
-    }
-    return;
-  }
-  for (int g = (cw + NCW - rot) % NCW; g < ng32; g += NCW) {
-    const int row = g * 32 + lane;
-    if (row >= rows) continue;
-    const uint8_t* rp = row_ptr<VAR>(tv, row);
-    uint64_t hx       = static_cast<uint64_t>(hs->seed);
-    uint32_t hm       = static_cast<uint32_t>(hs->seed);
-    uint32_t hh       = 0;
-    for (int k = 0; k < nkeys; ++k) {
-      const int c      = hs->key_col[k];
-      const bool valid = (rp[voff + (c >> 3)] >> (c & 7)) & 1u;
-      const int32_t ty = hs->key_type[k];
-      const int sz     = key_size(ty);
-      uint64_t v = 0, v2 = 0;
-      if (valid) {
-        v = load_key<SAFE>(rp + hs->key_start[k], sz);
-        if (sz == 16) v2 = load_key<SAFE>(rp + hs->key_start[k] + 8, 8);
-      }
-      if (kind == SRJ_HASH_XXHASH64) {
-        if (valid) hx = hash::xx_fixed(ty, v, v2, hx);
-      } else if (kind == SRJ_HASH_MURMUR3_32) {
-        if (valid) hm = hash::mm_fixed(ty, v, v2, hm);
-      } else {
-        hh = 31u * hh + (valid ? static_cast<uint32_t>(hash::hive_fixed(ty, v)) : 0u);
-      }
-    }
-    if (kind == SRJ_HASH_XXHASH64)
-      reinterpret_cast<uint64_t*>(hs->out)[r0 + row] = hx;
-    else if (kind == SRJ_HASH_MURMUR3_32)
-      reinterpret_cast<uint32_t*>(hs->out)[r0 + row] = hm;
-    else
-      reinterpret_cast<uint32_t*>(hs->out)[r0 + row] = hh;
-  }
-}
-
 // Variable-width tables: does every row place its strings where convert_to_rows would (chars of the
 // STRING columns back to back, in column order, from byte size_per_row -- RC:838-858)?  Phase 2's fast
 // path relies on it; a mismatch only flips a status bit that routes phase 2 to the generic gather.
@@ -470,7 +328,6 @@ __device__ __forceinline__ void process_tile(const FromRowsParams& p, const Smem
   transpose_class<2, NCW, RPL, VAR, PRED, SAFE, ONEG>(p, t, ws, tv, 1);
   transpose_class<1, NCW, RPL, VAR, PRED, SAFE, ONEG>(p, t, ws, tv, 0);
   validity_tile<NCW, VAR, PRED, SAFE>(p, t, ws, tv);
-  if (t.hash) hash_tile<NCW, VAR, SAFE>(t.hash, tv.base, tv.s_off, tv.stride, tv.r0, tv.rows, cw);
   if constexpr (VAR) {
     if (p.status && p.nstr > 0)
       canonical_check_tile<NCW, SAFE>(tv.base, tv.s_off, tv.rows, cw, t.string_start, p.nstr, p.size_per_row, p.status);
@@ -681,7 +538,6 @@ __global__ void __launch_bounds__((NCW + 1) * 32, 1) from_rows_kernel(const __gr
   int32_t* s_nulls     = reinterpret_cast<int32_t*>(s_masks + p.ncols);
   int32_t* s_next_off  = s_nulls + ((p.ncols + 3) & ~3);  // producer scratch: offsets of the NEXT tile
   int32_t* s_str_start = s_next_off + ((p.tile_rows + 4) & ~3);
-  HashSpec* s_hash     = reinterpret_cast<HashSpec*>(s_str_start + ((p.nstr + 3) & ~3));  // 16-byte aligned
 
   const int tid = threadIdx.x;
   for (int i = tid; i < p.nentries; i += kThreads) {
@@ -693,21 +549,6 @@ __global__ void __launch_bounds__((NCW + 1) * 32, 1) from_rows_kernel(const __gr
     s_nulls[i] = 0;
   }
   for (int i = tid; i < p.nstr; i += kThreads) s_str_start[i] = p.string_start[i];
-  if (tid == 0 && p.hash_kind != SRJ_HASH_NONE) {
-    s_hash->kind            = p.hash_kind;
-    s_hash->nkeys           = p.hash_nkeys;
-    s_hash->validity_offset = p.validity_offset;
-    s_hash->seed            = p.hash_seed;
-    s_hash->out             = p.hash_out;
-    int plain               = p.hash_kind == SRJ_HASH_XXHASH64 || p.hash_kind == SRJ_HASH_MURMUR3_32;
-    for (int k = 0; k < p.hash_nkeys; ++k) plain &= plain_key_bytes(p.key_type[k]) != 0;
-    s_hash->plain = plain;
-    for (int k = 0; k < 16; ++k) {
-      s_hash->key_start[k] = p.key_start[k];
-      s_hash->key_type[k]  = p.key_type[k];
-      s_hash->key_col[k]   = p.key_col[k];
-    }
-  }
   if (tid == 0) {
     for (int s = 0; s < NS; ++s) {
       mbar_init(&full[s], 1);
@@ -745,8 +586,7 @@ __global__ void __launch_bounds__((NCW + 1) * 32, 1) from_rows_kernel(const __gr
   } else {
     // =================================== consumers ===================================
     const int cw = warp_id() - 1;
-    SmemTables t{s_ent_start, s_ent_dst, s_masks, p.null_counts ? s_nulls : nullptr, s_str_start,
-                 p.hash_kind != SRJ_HASH_NONE ? s_hash : nullptr};
+    SmemTables t{s_ent_start, s_ent_dst, s_masks, p.null_counts ? s_nulls : nullptr, s_str_start};
     WarpSched ws;
 #pragma unroll
     for (int k = 0; k < kNumClasses; ++k) ws.ustart[k] = (cw + NCW - (p.cls_ubase[k] % NCW)) % NCW;
@@ -807,7 +647,6 @@ size_t from_rows_smem_bytes(const Tiling& tl, int nentries, int ncols, int nstr)
   b += static_cast<size_t>(nentries) * 8 + static_cast<size_t>(ncols) * 8 + static_cast<size_t>((ncols + 3) & ~3) * 4;
   b += static_cast<size_t>((tl.tile_rows + 4) & ~3) * 4;
   b += static_cast<size_t>(nstr + 4) * 4;
-  b += sizeof(HashSpec) + 16;
   return (b + 127) & ~size_t{127};
 }
 
@@ -836,7 +675,7 @@ static int launch_variant(const FromRowsParams& p, unsigned grid, size_t smem, c
 
 int launch_from_rows(const srj_plan* plan, const uint8_t* rows, const int32_t* row_offsets, int64_t rows_bytes,
                      int64_t num_rows, void* const* d_ent_dst, uint32_t* const* d_masks, int64_t* d_null_counts,
-                     int64_t* d_status, const srj_fused_hash* fh, cudaStream_t stream)
+                     int64_t* d_status, cudaStream_t stream)
 {
   if (num_rows == 0) return SRJ_OK;
   FromRowsParams p{};
@@ -880,41 +719,19 @@ int launch_from_rows(const srj_plan* plan, const uint8_t* rows, const int32_t* r
   p.size_per_row = plan->size_per_row;
   p.string_start = plan->d_string_start;
   p.status       = reinterpret_cast<unsigned long long*>(d_status);
-  p.hash_kind    = SRJ_HASH_NONE;
-  if (fh && fh->kind != SRJ_HASH_NONE) {
-    p.hash_kind  = fh->kind;
-    p.hash_nkeys = fh->num_keys;
-    p.hash_seed  = fh->seed;
-    p.hash_out   = fh->out;
-    for (int k = 0; k < fh->num_keys; ++k) {
-      const int c    = fh->key_columns[k];
-      p.key_col[k]   = c;
-      p.key_type[k]  = plan->type_ids[c];
-      p.key_start[k] = plan->col_start[c];
-    }
-  }
   int dev = 0, nsm = 0;
   SRJ_CUDA_TRY(cudaGetDevice(&dev));
   SRJ_CUDA_TRY(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
   // super-tile = a multiple of the tile height (=> of 32 or 8|16: mask-byte aligned).  Fixed-stride
   // tables: two tiles (faster than one, flat beyond).  Variable-width tables cut tiles adaptively inside a
   // super-tile of >= 4 tiles so the last, shorter tile of a super-tile is amortised.
-  const int sup_tiles_env = SRJ_KNOB("SRJ_FR_SUPER", 0);
-  const int64_t T  = p.tile_rows;
-  int sup_tiles    = row_offsets ? 8 : 2;
-  if (sup_tiles_env > 0) sup_tiles = sup_tiles_env;
-  p.super_rows     = T * sup_tiles;
-  const int64_t ns = (num_rows + p.super_rows - 1) / p.super_rows;
-  int64_t grid     = std::min<int64_t>(nsm, ns);
-  const size_t smem    = from_rows_smem_bytes(plan->tiling, p.nentries, p.ncols, plan->num_string_columns);
-  const int variant = SRJ_KNOB("SRJ_FR_VARIANT", 0);
-  int rc;
-  switch (variant) {
-    case 2: rc = launch_variant<7>(p, static_cast<unsigned>(grid), smem, stream); break;
-    // 11 consumer warps: 384 threads x 168 registers fills the register file with no spills (15 warps cap
-    // the kernel at 128 registers and spill inside the transpose loop)
-    default: rc = launch_variant<11>(p, static_cast<unsigned>(grid), smem, stream); break;
-  }
+  p.super_rows      = static_cast<int64_t>(p.tile_rows) * (row_offsets ? 8 : 2);
+  const int64_t ns  = (num_rows + p.super_rows - 1) / p.super_rows;
+  const int64_t grid = std::min<int64_t>(nsm, ns);
+  const size_t smem = from_rows_smem_bytes(plan->tiling, p.nentries, p.ncols, plan->num_string_columns);
+  // 11 consumer warps: 384 threads x 168 registers fills the register file with no spills (15 warps cap
+  // the kernel at 128 registers and spill inside the transpose loop)
+  const int rc = launch_variant<11>(p, static_cast<unsigned>(grid), smem, stream);
   if (rc != SRJ_OK) return rc;
   SRJ_CUDA_TRY(cudaGetLastError());
   return SRJ_OK;

@@ -576,8 +576,7 @@ __global__ void __launch_bounds__((NCW + kWProducers) * 32, 1) from_rows_wide_ke
 // ---- scan over the 32-row group totals ----------------------------------------------------------------
 // base[c][g] <- chars of column c before 32-row group g (exclusive scan of the group totals), in the caller's
 // workspace.  The offsets arrays keep the inclusive sums inside each group that from_rows_wide_kernel wrote; phase 2
-// (strings.cu) adds the group base while it gathers, wide_finalize_offsets_kernel does it when phase 1 is asked for
-// finished offsets.
+// (strings.cu) adds the group base while it gathers.
 constexpr int kGsThreads = 256;
 constexpr int kGsPer     = 16;                    // groups per thread
 constexpr int kGsChunk   = kGsThreads * kGsPer;   // groups per CTA
@@ -690,17 +689,6 @@ __global__ void __launch_bounds__(kGsThreads) wide_group_scan_kernel(const __gri
   if (threadIdx.x == 0) char_totals[q.ncols] = (*reinterpret_cast<volatile uint32_t*>(&q.sync_words[1])) | (bad ? 1u : 0u);
 }
 
-// group-local inclusive sums -> absolute offsets, for consumers that want finished offsets after phase 1
-__global__ void __launch_bounds__(256) wide_finalize_offsets_kernel(const __grid_constant__ WideScanTab tab, const uint32_t* base,
-                                                                     int64_t ngroups, int64_t num_rows)
-{
-  int32_t* offs   = tab.offs[blockIdx.y];
-  const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;  // position 0..n
-  if (i > num_rows) return;
-  if (i == 0) { offs[0] = 0; return; }
-  offs[i] += static_cast<int32_t>(base[static_cast<int64_t>(blockIdx.y) * ngroups + ((i - 1) >> 5)]);
-}
-
 // ---- host side -----------------------------------------------------------------------------------------
 // Plans the slabs of a schema.  Returns false (wide.enabled stays false) when the schema is not a wide
 // variable-width table or the kernel's tables would not fit shared memory.
@@ -710,10 +698,8 @@ bool plan_wide(srj_plan* plan)
   wp.enabled   = false;
   const int nc = plan->num_columns, nstr = plan->num_string_columns;
   const int spr      = plan->size_per_row;
-  const int min_spr  = SRJ_KNOB("SRJ_W_MINROW", 512);
-  const int min_nstr = SRJ_KNOB("SRJ_W_MINSTR", 8);
-  if (nstr < min_nstr || spr < min_spr || nc > kWMaxCols) return false;
-  const int slab_cap = SRJ_KNOB("SRJ_W_SLABCAP", 3200);
+  if (nstr < 8 || spr < 512 || nc > kWMaxCols) return false;
+  const int slab_cap = 3200;
   int nslabs         = (spr + slab_cap - 1) / slab_cap;
   nslabs             = std::max(1, std::min(nslabs, 16));
   // first column of each slab: the first one starting at or after i * spr / nslabs
@@ -766,8 +752,7 @@ bool plan_wide(srj_plan* plan)
                         static_cast<size_t>(nslabs) * 6 * 16 * 2 + 256;
   const size_t budget = 232448;
   if (tables > 64 * 1024) return false;
-  int NS = SRJ_KNOB("SRJ_W_STAGES", 3);
-  NS     = std::max(2, std::min(NS, kWMaxStages));
+  int NS = 3;  // two when three would leave tiles of fewer than 64 rows
   int R  = 0;
   for (;;) {
     const size_t avail = budget - tables;
@@ -777,7 +762,6 @@ bool plan_wide(srj_plan* plan)
     --NS;
   }
   R = std::min(R, 32 * kWMaxG);
-  if (const int r = SRJ_KNOB("SRJ_W_ROWS", 0)) R = std::min(R, r / 32 * 32);
   if (R < 32) return false;
   wp.R       = R;
   wp.G       = R / 32;
@@ -839,7 +823,7 @@ static int launch_wide_variant(const WideParams& p, const WidePtrTab& tab, unsig
 // cols: the caller's output columns (host array).  d_scratch: the call pair's workspace (wide_workspace_bytes()).
 int launch_from_rows_wide(const srj_plan* plan, const uint8_t* rows, const int32_t* row_offsets, int64_t rows_bytes,
                           int64_t num_rows, const srj_column* cols, int64_t* d_null_counts, int64_t* d_char_totals,
-                          void* d_scratch, bool finalize, cudaStream_t stream)
+                          void* d_scratch, cudaStream_t stream)
 {
   if (num_rows == 0) return SRJ_OK;
   const WidePlan& wp = plan->wide;
@@ -847,7 +831,6 @@ int launch_from_rows_wide(const srj_plan* plan, const uint8_t* rows, const int32
   int dev = 0, nsm = 0;
   SRJ_CUDA_TRY(cudaGetDevice(&dev));
   SRJ_CUDA_TRY(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
-  if (const int g = SRJ_KNOB("SRJ_W_GRID", 0)) nsm = std::min(nsm, g);
   const int64_t ntiles = (num_rows + wp.R - 1) / wp.R;
   const unsigned grid  = static_cast<unsigned>(std::min<int64_t>(std::min(nsm, kWMaxGrid), ntiles));
   WidePtrTab tab;
@@ -888,12 +871,7 @@ int launch_from_rows_wide(const srj_plan* plan, const uint8_t* rows, const int32
   p.bad_part        = p.null_part + static_cast<size_t>(kWMaxGrid) * nc;
   p.sync_words      = reinterpret_cast<uint32_t*>(p.bad_part + kWMaxGrid);
   const size_t smem = wide_smem_bytes(plan);
-  int rc;
-  switch (SRJ_KNOB("SRJ_W_WARPS", 12)) {
-    case 8: rc = launch_wide_variant<8>(p, tab, grid, smem, stream); break;
-    case 16: rc = launch_wide_variant<16>(p, tab, grid, smem, stream); break;
-    default: rc = launch_wide_variant<12>(p, tab, grid, smem, stream); break;
-  }
+  const int rc = launch_wide_variant<12>(p, tab, grid, smem, stream);
   if (rc != SRJ_OK) return rc;
   WideScanParams q{};
   q.agg         = p.agg;
@@ -911,10 +889,6 @@ int launch_from_rows_wide(const srj_plan* plan, const uint8_t* rows, const int32
   for (int s2 = 0; s2 < nstr; ++s2) q.str_bits[plan->string_columns[s2] >> 6] |= 1ull << (plan->string_columns[s2] & 63);
   const int64_t nchunks = (p.ngroups + kGsChunk - 1) / kGsChunk;
   wide_group_scan_kernel<<<dim3(static_cast<unsigned>(nchunks), nstr), kGsThreads, 0, stream>>>(q, stab);
-  if (finalize) {
-    const unsigned gx = static_cast<unsigned>((num_rows + 1 + 255) / 256);
-    wide_finalize_offsets_kernel<<<dim3(gx, nstr), 256, 0, stream>>>(stab, d_base, p.ngroups, num_rows);
-  }
   SRJ_CUDA_TRY(cudaGetLastError());
   return SRJ_OK;
 }

@@ -383,7 +383,7 @@ __global__ void __launch_bounds__(kHsThreads, 1) row_hash_stream_kernel(const __
 static int launch_hash_stream(int kind, const HashParams& hp, int64_t num_rows, cudaStream_t stream, int64_t* done)
 {
   *done = 0;
-  if (SRJ_KNOB("SRJ_HASH_NOSTREAM", 0) || hp.ncols > kHsMaxCols || num_rows < 4 * kHsRows) return SRJ_OK;
+  if (hp.ncols > kHsMaxCols || num_rows < 4 * kHsRows) return SRJ_OK;
   HsParams p{};
   int off = 0;
   for (int c = 0; c < hp.ncols; ++c) {
@@ -403,7 +403,6 @@ static int launch_hash_stream(int kind, const HashParams& hp, int64_t num_rows, 
   p.out         = hp.out;
   p.stage_bytes = (off + 127) & ~127;
   p.nstages     = std::min<int>(kHsMaxStages, (200 * 1024) / p.stage_bytes);
-  if (const int ns = SRJ_KNOB("SRJ_HASH_STAGES", 0)) p.nstages = std::min(p.nstages, ns);
   if (p.nstages < 2) return SRJ_OK;
   p.nchunks = num_rows / kHsRows;
   int dev = 0, nsm = 0;
@@ -491,7 +490,7 @@ int launch_hash(int kind, const srj_column* cols, int32_t num_columns, int64_t n
       }
     }
     const unsigned grid = static_cast<unsigned>((p.n + per_block - 1) / per_block);
-    bool plain = SRJ_KNOB("SRJ_HASH_GENERAL", 0) == 0;
+    bool plain = true;
     for (int i = 0; i < p.ncols; ++i) plain = plain && p.cols[i].kind != 0;
     if (plain) {
       // persistent launch: as many CTAs as stay resident (the kernel strides over the row blocks)
@@ -512,9 +511,8 @@ int launch_hash(int kind, const srj_column* cols, int32_t num_columns, int64_t n
           SRJ_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, row_hash_plain_kernel<SRJ_HASH_HIVE>, kHashThreads, 0));
         occ_cache[kind & 3] = occ = std::max(1, occ);
       }
-      const int e_w        = SRJ_KNOB("SRJ_HASH_WAVES", -1);  // tuning knob (development builds): CTAs per SM, 0 = one CTA per row block
-      const int waves      = e_w >= 0 ? e_w : std::max(1, occ) * (kind == SRJ_HASH_HIVE ? 1 : 4);
-      const unsigned pgrid = waves > 0 ? std::min<unsigned>(grid, static_cast<unsigned>(nsm * waves)) : grid;
+      const int waves      = occ * (kind == SRJ_HASH_HIVE ? 1 : 4);  // CTAs per SM
+      const unsigned pgrid = std::min<unsigned>(grid, static_cast<unsigned>(nsm * waves));
       if (kind == SRJ_HASH_XXHASH64)
         row_hash_plain_kernel<SRJ_HASH_XXHASH64><<<pgrid, kHashThreads, 0, stream>>>(p);
       else if (kind == SRJ_HASH_MURMUR3_32)

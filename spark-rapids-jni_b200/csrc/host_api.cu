@@ -83,8 +83,7 @@ int from_rows_host_fixed(const srj_plan* plan, ArenaLease& L, const uint8_t* h_r
   if (chunk_rows <= 0) {
     // ~1/12 of the input per chunk, between 32 MB and 1 GB of rows (larger chunks are faster): per chunk the copies
     // have a fixed cost and the first H2D / last D2H are not overlapped
-    int64_t cbytes = std::min<int64_t>(1ll << 30, std::max<int64_t>(32ll << 20, num_rows * S / 12));
-    if (const int mb = SRJ_KNOB("SRJ_HOST_CHUNK_MB", 0)) cbytes = static_cast<int64_t>(mb) << 20;
+    const int64_t cbytes = std::min<int64_t>(1ll << 30, std::max<int64_t>(32ll << 20, num_rows * S / 12));
     chunk_rows = std::max<int64_t>(32 * 1024, cbytes / S);
   }
   const int64_t T = plan->tiling.tile_rows >= 32 ? plan->tiling.tile_rows : 32;
@@ -130,8 +129,7 @@ int from_rows_host_fixed(const srj_plan* plan, ArenaLease& L, const uint8_t* h_r
     uint8_t* d_cols   = L.buf(1) + col_bytes * s;
     SRJ_CUDA_TRY(cudaMemcpyAsync(d_rows, h_rows + r0 * S, static_cast<size_t>(n) * S, cudaMemcpyHostToDevice, st));
     // the kernel sees a chunk-local table whose last mask word is zero-tailed; chunk starts are multiples of 32
-    rc = launch_from_rows(plan, d_rows, nullptr, n * S, n, d_tab, reinterpret_cast<uint32_t* const*>(d_tab + nent), d_nulls, nullptr,
-                          nullptr, st);
+    rc = launch_from_rows(plan, d_rows, nullptr, n * S, n, d_tab, reinterpret_cast<uint32_t* const*>(d_tab + nent), d_nulls, nullptr, st);
     if (rc != SRJ_OK) return rc;
     for (int c = 0; c < nc; ++c) {
       SRJ_CUDA_TRY(cudaMemcpyAsync(static_cast<uint8_t*>(h_cols[c].data) + r0 * plan->col_size[c], d_cols + off_data[c],

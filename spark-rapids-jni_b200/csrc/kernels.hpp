@@ -11,27 +11,26 @@ namespace srj {
 // from_rows.cu
 int launch_from_rows(const srj_plan* plan, const uint8_t* rows, const int32_t* row_offsets, int64_t rows_bytes,
                      int64_t num_rows, void* const* d_ent_dst, uint32_t* const* d_masks, int64_t* d_null_counts,
-                     int64_t* d_status, const srj_fused_hash* fh, cudaStream_t stream);
+                     int64_t* d_status, cudaStream_t stream);
 
 size_t from_rows_smem_bytes(const Tiling& tl, int nentries, int ncols, int nstr);  // dynamic shared memory of from_rows_kernel
 
 // from_rows_wide.cu: wide variable-width tables (per-row TMA slabs; offsets leave as group-local inclusive sums +
-// absolute group bases unless `finalize`)
+// absolute group bases, finished by phase 2)
 bool plan_wide(srj_plan* plan);
 int64_t wide_workspace_bytes(const srj_plan* plan, int64_t num_rows);
 const uint32_t* wide_workspace_bases(const srj_plan* plan, int64_t num_rows, const void* workspace);  // [nstr][ngroups]
 int launch_from_rows_wide(const srj_plan* plan, const uint8_t* rows, const int32_t* row_offsets, int64_t rows_bytes,
                           int64_t num_rows, const srj_column* cols /* host array of the output columns */,
                           int64_t* d_null_counts, int64_t* d_char_totals, void* d_scratch /* wide_workspace_bytes() */,
-                          bool finalize, cudaStream_t stream);
+                          cudaStream_t stream);
 
 // strings.cu
 // In-place inclusive scan of the int32 lengths stored at offsets[c][1..n] for every STRING column
 // (offsets[c][0] = 0), per-column totals to d_char_totals[schema col] (int64), a total beyond INT32_MAX sets bit 1 of *d_status.
 int launch_string_offsets_scan(int32_t* const* d_offsets /* device array [nstr] */, const int32_t* d_string_cols,
                                int nstr, int64_t num_rows, int64_t* d_char_totals, int64_t* d_status,
-                               void* d_partials /* int64 [nstr * nchunks] */,
-                               bool mark_finished /* set bit 2 of *d_status: the offsets are complete */, cudaStream_t stream);
+                               void* d_partials /* int64 [nstr * nchunks] */, cudaStream_t stream);
 int64_t string_scan_partials_bytes(int nstr, int64_t num_rows);
 // copy_strings_from_rows replacement.  cols = the caller's columns (host array); d_tab = device table
 // [offsets nstr][chars nstr], needed (and uploaded by the caller) only when !strings_fast_path().

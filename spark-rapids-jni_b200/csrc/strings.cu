@@ -54,7 +54,7 @@ __global__ void __launch_bounds__(kScanThreads) scan_partials_kernel(int32_t* co
 // exclusive scan of each column's chunk sums, in place; writes the column total
 __global__ void __launch_bounds__(kScanThreads) scan_chunks_kernel(int64_t* partials, int nchunks,
                                                                     const int32_t* string_cols, int64_t* char_totals,
-                                                                    unsigned long long* status, int mark_finished)
+                                                                    unsigned long long* status)
 {
   __shared__ int64_t s_warp[kScanThreads / 32];
   __shared__ int64_t s_carry;
@@ -86,8 +86,6 @@ __global__ void __launch_bounds__(kScanThreads) scan_chunks_kernel(int64_t* part
     const int64_t total = s_carry;
     if (char_totals) char_totals[string_cols[c]] = total;
     if (total > INT32_MAX && status) atomicOr(status, 2ull);  // cudf strings offsets are int32: bit 1 of the status word
-    // bit 2: the offsets are finished (a wide plan whose phase 1 ran this whole-row path, e.g. with a fused hash)
-    if (mark_finished && status && c == 0) atomicOr(status, 4ull);
   }
 }
 
@@ -143,8 +141,7 @@ int64_t string_scan_partials_bytes(int nstr, int64_t num_rows)
 }
 
 int launch_string_offsets_scan(int32_t* const* d_offsets, const int32_t* d_string_cols, int nstr, int64_t num_rows,
-                               int64_t* d_char_totals, int64_t* d_status, void* d_partials, bool mark_finished,
-                               cudaStream_t stream)
+                               int64_t* d_char_totals, int64_t* d_status, void* d_partials, cudaStream_t stream)
 {
   if (nstr == 0) return SRJ_OK;
   const int64_t n1  = num_rows + 1;
@@ -153,7 +150,7 @@ int launch_string_offsets_scan(int32_t* const* d_offsets, const int32_t* d_strin
   dim3 grid(nchunks, nstr);
   scan_partials_kernel<<<grid, kScanThreads, 0, stream>>>(d_offsets, n1, nchunks, partials);
   scan_chunks_kernel<<<nstr, kScanThreads, 0, stream>>>(partials, nchunks, d_string_cols, d_char_totals,
-                                                        reinterpret_cast<unsigned long long*>(d_status), mark_finished ? 1 : 0);
+                                                        reinterpret_cast<unsigned long long*>(d_status));
   scan_apply_kernel<<<grid, kScanThreads, 0, stream>>>(d_offsets, n1, nchunks, partials);
   SRJ_CUDA_TRY(cudaGetLastError());
   return SRJ_OK;
@@ -339,10 +336,8 @@ __device__ __forceinline__ void generic_gather(const uint8_t* __restrict__ rows,
 __global__ void __launch_bounds__(kStrWarps * 32) strings_from_rows_kernel(
   const uint8_t* __restrict__ rows, const int32_t* __restrict__ row_offsets, int64_t row_stride, int64_t num_rows,
   int nstr, const int32_t* __restrict__ string_start, int32_t* const* __restrict__ offsets,
-  uint8_t* const* __restrict__ chars, int64_t ntiles, const int64_t* __restrict__ status, const uint32_t* bases)
+  uint8_t* const* __restrict__ chars, int64_t ntiles, const uint32_t* bases)
 {
-  // status bit 2: phase 1 already left finished offsets (ignore the group bases)
-  if (status && (*status & 4)) bases = nullptr;
   __shared__ __align__(16) uint8_t s_line[kStrWarps * kStrLine];
   generic_gather(rows, row_offsets, row_stride, num_rows, nstr, string_start, offsets, chars, ntiles, bases,
                  static_cast<int64_t>(blockIdx.x) * kStrWarps + warp_id(), static_cast<int64_t>(gridDim.x) * kStrWarps,
@@ -461,7 +456,7 @@ __global__ void __launch_bounds__(kSwMaxThreads, 1) strings_wide_kernel(const __
     if (warp_id() == 0) return;
     const int ncons = (blockDim.x >> 5) - 1;
     generic_gather(p.rows, p.row_offsets, p.fixed_row_size, p.num_rows, p.nstr, p.string_start, s_offs, s_chars,
-                   (p.num_rows + 31) >> 5, (*p.status & 4) ? nullptr : p.bases,
+                   (p.num_rows + 31) >> 5, p.bases,
                    static_cast<int64_t>(blockIdx.x) * ncons + (warp_id() - 1),
                    static_cast<int64_t>(gridDim.x) * ncons, smem_u32(stg0 + static_cast<size_t>(warp_id() - 1) * kSwLine));
     return;
@@ -552,7 +547,7 @@ __global__ void __launch_bounds__(kSwMaxThreads, 1) strings_wide_kernel(const __
     const int c0         = wi * p.cpw;
     const int ncol       = tmax(0, tmin(p.nstr, c0 + p.cpw) - c0);
     const uint32_t stg_s = smem_u32(stg0 + static_cast<size_t>(cw) * kSwLine);
-    const bool semi      = p.bases != nullptr && !(p.status && (*p.status & 4));  // bit 2: phase 1 left finished offsets
+    const bool semi      = p.bases != nullptr;  // offsets hold group-local sums: finish them here
     for (int it = gi, k = 0;; it += kSwNG, ++k) {
       const int s        = it % NS;
       const uint32_t par = (it / NS) & 1;
@@ -653,7 +648,7 @@ static size_t strings_wide_smem_bytes(int nstr, int stage_bytes, int wpt)
 bool strings_wide_eligible(const srj_plan* plan)
 {
   const int nstr = plan->num_string_columns;
-  return nstr >= SRJ_KNOB("SRJ_SW_MINCOLS", 8) && nstr <= kSwMaxWpt * kSwMaxCpw;
+  return nstr >= 8 && nstr <= kSwMaxWpt * kSwMaxCpw;
 }
 
 // the fast gather needs phase 1's status word (it tells canonical rows from the rest)
@@ -697,12 +692,9 @@ int launch_strings_from_rows(const srj_plan* plan, const uint8_t* rows, const in
     const int64_t avg_var   = std::max<int64_t>(0, rows_bytes / num_rows - plan->size_per_row) + 16;
     int64_t stage           = (avg_var * 32 * 5 / 4 + 1023) & ~int64_t{1023};
     stage                   = std::max<int64_t>(4096, std::min(stage, cap));
-    if (const int kb = SRJ_KNOB("SRJ_SW_STAGE_KB", 0)) stage = std::min<int64_t>(cap, static_cast<int64_t>(kb) * 1024);
     p.stage_bytes           = static_cast<int32_t>(stage);
     const int64_t ntiles    = (num_rows + 31) / 32;
-    int nsm_b               = nsm;
-    if (const int g = SRJ_KNOB("SRJ_SW_GRID", 0)) nsm_b = std::min(nsm, g);
-    const int64_t grid      = std::min<int64_t>(nsm_b, ntiles);
+    const int64_t grid      = std::min<int64_t>(nsm, ntiles);
     const size_t smem       = strings_wide_smem_bytes(nstr, p.stage_bytes, p.wpt);
     SRJ_CUDA_TRY(cudaFuncSetAttribute(strings_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
     strings_wide_kernel<<<static_cast<unsigned>(grid), (1 + kSwNG * p.wpt) * 32, smem, stream>>>(p);
@@ -714,7 +706,7 @@ int launch_strings_from_rows(const srj_plan* plan, const uint8_t* rows, const in
   const int64_t grid   = std::min<int64_t>(ntiles, static_cast<int64_t>(nsm) * 8);
   strings_from_rows_kernel<<<static_cast<unsigned>(grid), kStrWarps * 32, 0, stream>>>(
     rows, row_offsets, plan->fixed_row_size, num_rows, nstr, plan->d_string_start, reinterpret_cast<int32_t* const*>(d_tab),
-    reinterpret_cast<uint8_t* const*>(d_tab + nstr), ntiles, d_status, d_bases);
+    reinterpret_cast<uint8_t* const*>(d_tab + nstr), ntiles, d_bases);
   SRJ_CUDA_TRY(cudaGetLastError());
   return SRJ_OK;
 }

@@ -882,7 +882,7 @@ int launch_to_rows(const srj_plan* plan, const void* const* d_col_data, const ui
   const int S = plan->fixed_row_size;
   int D       = 0;
   for (int sz : plan->col_size) D += sz;
-  bool fast = plan->num_string_columns == 0 && plan->d_tr_chunk_off != nullptr && SRJ_KNOB("SRJ_TR_GENERIC", 0) == 0;
+  bool fast = plan->num_string_columns == 0 && plan->d_tr_chunk_off != nullptr;
   int R = 0, NS = 3;
   if (fast) {
     // smem: NS staging stages of R*D bytes + 2 row images of R*S bytes (+ tables)
@@ -974,12 +974,8 @@ static int launch_to_rows_generic(const srj_plan* plan, const void* const* d_col
   // many resident CTAs rather than deep buffering: variable-width tables use ONE 40 KB stage per CTA
   // (4-5 CTAs per SM); fixed-width tails keep two 48 KB stages.
   const bool var        = plan->num_string_columns > 0;
-  const int env_stage_kb = SRJ_KNOB("SRJ_TR_STAGE_KB", 0);
-  const int env_nbuf     = SRJ_KNOB("SRJ_TR_NBUF", 0);
   int stage_bytes       = (var ? 44 : 48) * 1024;
   int nbuf              = var ? 1 : 2;
-  if (env_stage_kb > 0) stage_bytes = env_stage_kb * 1024;
-  if (env_nbuf > 0) nbuf = env_nbuf;
   int tile_rows         = (stage_bytes / plan->fixed_row_size) / 32 * 32;
   if (tile_rows > 512) tile_rows = 512;
   if (tile_rows < 32) tile_rows = (stage_bytes / plan->fixed_row_size) >= 16 ? 16 : 8;

@@ -5,7 +5,7 @@
 // consecutive rows -- and every shared-memory write lands in the lane's own row image):
 //
 // to_rows3_kernel (wide rows, >= ~3 KB: the C3 shape).  One CTA of 24 warps per SM owning a ~150-200 KB row-image
-// buffer (variant: two CTAs of 12 warps).  A tile = as many rows (<= 32) as fit.  Per tile:
+// buffer.  A tile = as many rows (<= 32) as fit.  Per tile:
 //   1. geometry from the LIST offsets (already written by batch_offsets_kernel), every warp redundantly;
 //   2. string block sums: warp b sums the lengths of its block of STRING columns per row and stages the tile's
 //      chars of those columns -- one contiguous global range per column -- into the column's shared-memory slot
@@ -517,7 +517,6 @@ __global__ void __launch_bounds__(kT3Warps * 32, kCtasPerSm) to_rows3_kernel(con
 // A tile whose rows do not fit the warp's buffer raises *fail_flag (generic kernel redoes the batch).
 // ==================================================================================================
 constexpr int kTwWarps = 24;
-constexpr bool kWarpKernelDefault = true;  // SRJ_TR_NOWARP=1 switches it off (development)
 
 struct ToRowsWParams {
   const void* const* col_data;
@@ -754,31 +753,20 @@ int launch_to_rows_var(const srj_plan* plan, const void* const* d_col_data, cons
   *launched = 0;
   const int nstr = plan->num_string_columns;
   if (nstr == 0 || row_count == 0 || !d_fail_flag || !h_col_data) return SRJ_OK;
-  if (SRJ_KNOB("SRJ_TR_GENERIC", 0)) return SRJ_OK;
-  const bool force = SRJ_KNOB("SRJ_TR_VAR_FORCE", 0) != 0;
   if ((reinterpret_cast<uintptr_t>(out_data) & 7) != 0) return SRJ_OK;
   for (const Entry& e : plan->tr_entries)
     if (reinterpret_cast<uintptr_t>(h_col_data[e.column]) & static_cast<uintptr_t>(plan->col_size[e.column] - 1)) return SRJ_OK;
 
-  {
-    // narrow rows: warp-private tiles (to_rows_w_kernel); wide rows: CTA tiles (to_rows3_kernel) below
-    const int64_t avg = std::max<int64_t>(plan->fixed_row_size, out_bytes / row_count);
-    if (!force && !SRJ_KNOB("SRJ_TR_NOWARP", 0) && (kWarpKernelDefault || SRJ_KNOB("SRJ_TR_WARP", 0))) {
-      const int rc = launch_to_rows_warp(plan, d_col_data, d_masks, d_str_offsets, d_str_chars, row_start, row_count, out_offsets,
-                                         out_data, avg, d_fail_flag, stream, launched);
-      if (rc != SRJ_OK || *launched) return rc;
-    }
-  }
+  // narrow rows: warp-private tiles (to_rows_w_kernel); wide rows: CTA tiles (to_rows3_kernel) below
+  const int64_t avg_row = std::max<int64_t>(plan->fixed_row_size, out_bytes / row_count);
+  const int rc = launch_to_rows_warp(plan, d_col_data, d_masks, d_str_offsets, d_str_chars, row_start, row_count, out_offsets,
+                                     out_data, avg_row, d_fail_flag, stream, launched);
+  if (rc != SRJ_OK || *launched) return rc;
   ToRows3Params p{};
   p.nfixed  = static_cast<int32_t>(plan->tr_entries.size());
   p.ncols   = plan->num_columns;
   p.nstr    = nstr;
-  const int env_sb = SRJ_KNOB("SRJ_T3_SB", 0);  // tuning knobs (development builds)
-  const int env_su = SRJ_KNOB("SRJ_T3_SUPER", 0);
-  const int env_w  = SRJ_KNOB("SRJ_T3_WARPS", 0);
-  const int nwarps = env_w == 12 ? 12 : 24;
-  const int cps    = nwarps == 24 ? 1 : 2;  // CTAs per SM
-  p.sb      = std::max(env_sb > 0 ? env_sb : (cps == 1 ? 4 : 8), (nstr + kT3MaxBlocks - 1) / kT3MaxBlocks);
+  p.sb      = std::max(4, (nstr + kT3MaxBlocks - 1) / kT3MaxBlocks);
   p.nblocks = (nstr + p.sb - 1) / p.sb;
   int nitems = p.nblocks + (p.ncols + 31) / 32;
   for (int k = 0; k < kNumClasses; ++k) {
@@ -790,17 +778,15 @@ int launch_to_rows_var(const srj_plan* plan, const void* const* d_col_data, cons
   const size_t tables = sizeof(void*) * (static_cast<size_t>(p.nfixed) + p.ncols + 2 * static_cast<size_t>(nstr)) +
                         4 * (static_cast<size_t>(p.nfixed) + nstr + 32 * static_cast<size_t>(p.nblocks) + nstr + 2 * static_cast<size_t>(nitems)) +
                         ((static_cast<size_t>(nitems) + 15) & ~size_t{15}) + 32 + 128;
-  const int64_t budget = 232448 / cps - 1024 - 64;
+  const int64_t budget = 232448 - 1024 - 64;
   // chars staging: a quarter of the budget at most, 1 KB per STRING column at most
   int64_t slot = std::min<int64_t>((budget - static_cast<int64_t>(tables)) / 4, 1024ll * nstr) / nstr / 16 * 16;
-  if (slot < 128 || SRJ_KNOB("SRJ_T3_NOSTAGE", 0)) slot = 0;
+  if (slot < 128) slot = 0;
   p.slot_bytes         = static_cast<int32_t>(slot);
   int64_t stage        = (budget - static_cast<int64_t>(tables) - slot * nstr) / 16 * 16;
   if (stage < 32 * 1024 || stage < 8ll * (plan->fixed_row_size + 64)) return SRJ_OK;
-  const int64_t avg_row = std::max<int64_t>(plan->fixed_row_size, out_bytes / row_count);
-  int fit               = static_cast<int>(std::min<int64_t>(32, stage / avg_row / 8 * 8));
-  if (!force && (fit < 8 || stage / avg_row >= 64)) return SRJ_OK;  // narrow rows: multi-group tiles of the generic kernel
-  if (fit < 8) fit = 8;
+  const int fit        = static_cast<int>(std::min<int64_t>(32, stage / avg_row / 8 * 8));
+  if (fit < 8 || stage / avg_row >= 64) return SRJ_OK;  // narrow rows: multi-group tiles of the generic kernel
 
   p.col_data        = d_col_data;
   p.masks           = d_masks;
@@ -813,7 +799,7 @@ int launch_to_rows_var(const srj_plan* plan, const void* const* d_col_data, cons
   p.validity_offset = plan->validity_offset;
   p.size_per_row    = plan->size_per_row;
   p.stage_bytes     = static_cast<int32_t>(stage);
-  p.super_rows      = fit * (env_su > 0 ? env_su : (cps == 1 ? 2 : 8));
+  p.super_rows      = fit * 2;
   for (int k = 0; k <= kNumClasses; ++k) p.class_begin[k] = plan->tr_class_begin[k];
   p.entries      = plan->d_tr_entries;
   p.string_start = plan->d_string_start;
@@ -823,16 +809,11 @@ int launch_to_rows_var(const srj_plan* plan, const void* const* d_col_data, cons
   SRJ_CUDA_TRY(cudaGetDevice(&dev));
   SRJ_CUDA_TRY(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
   const int64_t nsuper = (row_count + p.super_rows - 1) / p.super_rows;
-  const int64_t grid   = std::min<int64_t>(static_cast<int64_t>(cps) * nsm, nsuper);
+  const int64_t grid   = std::min<int64_t>(nsm, nsuper);
   const size_t smem    = static_cast<size_t>(stage) + 32 + static_cast<size_t>(slot) * nstr + tables;
   SRJ_CUDA_TRY(cudaMemsetAsync(d_fail_flag, 0, sizeof(int32_t), stream));
-  if (cps == 1) {
-    SRJ_CUDA_TRY(cudaFuncSetAttribute(to_rows3_kernel<24, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448 - 1024));
-    to_rows3_kernel<24, 1><<<static_cast<unsigned>(grid), 24 * 32, smem, stream>>>(p);
-  } else {
-    SRJ_CUDA_TRY(cudaFuncSetAttribute(to_rows3_kernel<12, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448 / 2 - 1024));
-    to_rows3_kernel<12, 2><<<static_cast<unsigned>(grid), 12 * 32, smem, stream>>>(p);
-  }
+  SRJ_CUDA_TRY(cudaFuncSetAttribute(to_rows3_kernel<24, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448 - 1024));
+  to_rows3_kernel<24, 1><<<static_cast<unsigned>(grid), 24 * 32, smem, stream>>>(p);
   SRJ_CUDA_TRY(cudaGetLastError());
   *launched = 1;
   return SRJ_OK;

@@ -79,6 +79,15 @@ def test_product_does_not_import_oracle():
                 assert "oracle" not in src.replace("test_product_does_not_import_oracle", ""), f"{f} mentions the oracle"
 
 
+def test_library_reads_no_environment():
+    """There is one build: no kernel variant or dispatch choice may hang on an environment variable."""
+    csrc = os.path.join(ROOT, "spark-rapids-jni_b200", "csrc")
+    for f in sorted(os.listdir(csrc)):
+        src = open(os.path.join(csrc, f), errors="replace").read()
+        assert not re.search(r"\bgetenv\b", src), f"{f} calls getenv"
+        assert "SRJ_KNOB" not in src, f"{f} mentions SRJ_KNOB"
+
+
 def test_library_holds_the_sm90a_kernels_and_tma_sass():
     """CPU-side evidence that the shipped .so is the hand-written sm_90a path: the kernels DESIGN.md §3.5 names are
     in the cubin, and their SASS uses the bulk-copy (TMA, UBLKCP) and cp.async (LDGSTS) instructions."""
