@@ -11,7 +11,7 @@ from util import cols_equal, random_table
 pytestmark = pytest.mark.gpu
 
 WIDE_SCHEMAS = {
-    # config C3 (3096-byte fixed section, 64 STRING columns, 3 slabs)
+    # config C3 (3096-byte fixed section, 64 STRING columns, one slab)
     "c3": [O.INT32, O.INT64, O.DECIMAL128, O.STRING] * 64,
     # odd alignments: 1/2-byte fields between strings, validity offset not a multiple of 4
     "odd": [O.INT8, O.STRING, O.INT16, O.DECIMAL128, O.STRING, O.INT64, O.BOOL8, O.INT32, O.STRING, O.FLOAT64, O.INT8] * 20,
@@ -20,7 +20,7 @@ WIDE_SCHEMAS = {
     "strings_first": [O.STRING] * 12 + [O.INT64] * 100,
     "strings_last": [O.INT64] * 100 + [O.STRING] * 12,
     "one_slab": [O.STRING, O.INT32] * 50,
-    # 6 slabs, 128 STRING columns
+    # 512 columns, 128 STRING columns: more than kWMaxCols, so the whole-row kernel serves it
     "c3x2": [O.INT32, O.INT64, O.DECIMAL128, O.STRING] * 128,
     # 9 STRING columns spread over 2 KB: exercises the "previous pair too far" planning fallback
     "sparse_strings": ([O.STRING] + [O.INT64] * 30) * 9,
@@ -207,7 +207,7 @@ def _check_to_rows(cols):
 
 WIDE_TO_ROWS = dict(WIDE_SCHEMAS)
 WIDE_TO_ROWS.update({
-    # several slabs whose cuts fall next to 16-byte fields
+    # 8 KB of 16-byte fields in front of 10 STRING columns
     "dec_slabs": [O.DECIMAL128] * 500 + [O.STRING] * 10,
     # size_per_row not a multiple of 8: the variable section starts inside an 8-byte store unit
     "phase": [O.INT64] * 70 + [O.STRING] * 9 + [O.INT8] * 3,
