@@ -351,11 +351,18 @@ __global__ void __launch_bounds__(kStrWarps * 32) strings_from_rows_kernel(
 // A tile is one 32-row group.  The CTA keeps kSwNG tiles in flight, each owned by a group of `wpt` consumer
 // warps; warp i of a group gathers the STRING columns [i * cpw, (i + 1) * cpw) of its tile.
 //
-//   producer warp : lane = row; one TMA bulk copy per row of JUST the row's variable section
+//   producer warps: lane = row; one TMA bulk copy per row of JUST the row's variable section
 //                   [offsets[r] + size_per_row, offsets[r + 1]) into a ring of 2 * kSwNG stages (two per
-//                   group), so the fixed section -- 79 % of a C3 row -- is never read by this phase;
+//                   group), so the fixed section -- 79 % of a C3 row -- is never read by this phase.  A copy costs
+//                   its issuing warp ~70 cycles, one lane at a time, so kSwProducers warps share the rows of a tile:
+//                   producer q issues the copies of the rows whose lane index is congruent to q and arrives on the
+//                   stage's full barrier with the bytes of its own copies.  Each one scans the tile's row offsets
+//                   itself (so they agree on the slots and on `direct`), and loads those of its NEXT tile while the
+//                   current tile's copies are issued;
 //   consumer warps: lane = row.  The warp reads its columns' offsets entries of the tile (one coalesced 128-byte
-//                   load per column), turns them into lengths, and the warps of the group exchange their
+//                   load per column; those of the group's next tile are loaded before it waits for the current
+//                   one, so that round trip overlaps the current tile's work), turns them into lengths, and the warps
+//                   of the group exchange their
 //                   per-row byte sums through shared memory (one named barrier per tile) to find where in the
 //                   row's variable section their first column starts.  Per column the lane's string moves as
 //                   aligned 32-bit words from the row image, funnel-shifted to the destination's byte
@@ -372,10 +379,11 @@ constexpr int kSwStages = 2 * kSwNG;
 constexpr int kSwFront  = 16;  // slack before a stage's payload (word reads may start up to 7 bytes early)
 constexpr int kSwBack   = 48;  // slack after it (word reads may run up to 44 bytes past a string)
 constexpr int kSwLine   = 16 + 1024 + 32;  // per-warp staging line
-constexpr int kSwMaxThreads = (1 + kSwNG * kSwMaxWpt) * 32;
+constexpr int kSwProducers  = 4;           // producer warps, one per scheduler (a power of two)
+constexpr int kSwMaxThreads = (kSwProducers + kSwNG * kSwMaxWpt) * 32;
+static_assert((kSwProducers & (kSwProducers - 1)) == 0 && kSwProducers <= 32, "kSwProducers: a power of two");
 
 struct SwHdr {
-  int64_t r0;
   int32_t rows;    // 0 = end
   int32_t direct;  // 1 = variable sections not staged (tile larger than a stage): read them from global memory
 };
@@ -444,7 +452,7 @@ __global__ void __launch_bounds__(kSwMaxThreads, 1) strings_wide_kernel(const __
   }
   if (tid == 0) {
     for (int s = 0; s < NS; ++s) {
-      mbar_init(&full[s], 1);
+      mbar_init(&full[s], kSwProducers);
       mbar_init(&empty[s], wpt);
     }
     fence_mbar_init();
@@ -453,12 +461,12 @@ __global__ void __launch_bounds__(kSwMaxThreads, 1) strings_wide_kernel(const __
   if (p.status && (*p.status & 1)) {
     // phase 1 saw rows that do not use the canonical layout: follow the stored pair offsets (RC:1143) with the generic
     // gather, every consumer warp of the grid taking (tile, column) tasks with its own staging line
-    if (warp_id() == 0) return;
-    const int ncons = (blockDim.x >> 5) - 1;
+    if (warp_id() < kSwProducers) return;
+    const int ncons = (blockDim.x >> 5) - kSwProducers;
+    const int cw    = warp_id() - kSwProducers;
     generic_gather(p.rows, p.row_offsets, p.fixed_row_size, p.num_rows, p.nstr, p.string_start, s_offs, s_chars,
-                   (p.num_rows + 31) >> 5, p.bases,
-                   static_cast<int64_t>(blockIdx.x) * ncons + (warp_id() - 1),
-                   static_cast<int64_t>(gridDim.x) * ncons, smem_u32(stg0 + static_cast<size_t>(warp_id() - 1) * kSwLine));
+                   (p.num_rows + 31) >> 5, p.bases, static_cast<int64_t>(blockIdx.x) * ncons + cw,
+                   static_cast<int64_t>(gridDim.x) * ncons, smem_u32(stg0 + static_cast<size_t>(cw) * kSwLine));
     return;
   }
 
@@ -466,33 +474,43 @@ __global__ void __launch_bounds__(kSwMaxThreads, 1) strings_wide_kernel(const __
   const uintptr_t b_hi = b_lo + static_cast<uintptr_t>(p.rows_bytes);
   const int64_t ntiles = (p.num_rows + 31) >> 5;
 
-  if (warp_id() == 0) {
-    // =================================== producer ===================================
+  if (warp_id() < kSwProducers) {
+    // =================================== producers ===================================
+    const int q     = warp_id();
+    const bool mine = (lane & (kSwProducers - 1)) == q;  // the rows whose copies this warp issues
+    uint32_t n0 = 0, n1 = 0;                             // row offsets [r, r + 1] of the lane's row of the next tile
+    auto load_offsets = [&](int64_t T) {
+      n0 = n1 = 0;
+      const int64_t r = (T << 5) + lane;
+      if (T < ntiles && r < p.num_rows) {
+        n0 = static_cast<uint32_t>(p.row_offsets[r]);
+        n1 = static_cast<uint32_t>(p.row_offsets[r + 1]);
+      }
+    };
+    load_offsets(blockIdx.x);
     int it = 0;
     for (int64_t T = blockIdx.x;; T += gridDim.x, ++it) {
       const int s        = it % NS;
       const uint32_t par = ((it / NS) & 1) ^ 1;
-      if (lane == 0) mbar_wait(&empty[s], par);
-      __syncwarp();
-      SwHdr* h = hdr0 + s;
+      SwHdr* h           = hdr0 + s;
       if (T >= ntiles) {
         // one end marker per group of consumer warps
         if (lane == 0) {
-          h->rows = 0;
+          mbar_wait(&empty[s], par);
+          if (q == 0) h->rows = 0;
           mbar_arrive(&full[s]);
         }
         if (T >= ntiles + static_cast<int64_t>(kSwNG - 1) * gridDim.x) break;
         continue;
       }
+      const int64_t o0 = n0, o1 = n1;
+      load_offsets(T + gridDim.x);  // in flight while this tile's copies are issued
+      if (lane == 0) mbar_wait(&empty[s], par);
+      __syncwarp();
       const int64_t r0 = T << 5;
       const int rows   = static_cast<int>(tmin<int64_t>(32, p.num_rows - r0));
       uint8_t* pay     = payload0 + static_cast<size_t>(s) * stage_span + kSwFront;
       int32_t* rowsm   = rowsm0 + s * 32;
-      int64_t o0 = 0, o1 = 0;
-      if (lane < rows) {
-        o0 = static_cast<uint32_t>(p.row_offsets[r0 + lane]);
-        o1 = static_cast<uint32_t>(p.row_offsets[r0 + lane + 1]);
-      }
       int64_t gs = o0 + p.size_per_row, ge = o1;
       if (ge < gs) ge = gs;
       const uintptr_t a_lo = b_lo + static_cast<uintptr_t>(gs);
@@ -515,7 +533,7 @@ __global__ void __launch_bounds__(kSwMaxThreads, 1) strings_wide_kernel(const __
       const bool over    = lane < rows && (x > p.stage_bytes || span >= (1 << 30));
       const bool direct  = __any_sync(0xffffffffu, over);
       uint32_t tx        = 0;
-      if (!direct && lane < rows) {
+      if (!direct && lane < rows && mine) {
         tx          = static_cast<uint32_t>(t_hi - t_lo);
         rowsm[lane] = slot + static_cast<int32_t>(a_lo - fl);
         // bytes of [a_lo, a_hi) outside the TMA window [t_lo, t_hi) (only at the ends of the buffer): by hand
@@ -526,14 +544,15 @@ __global__ void __launch_bounds__(kSwMaxThreads, 1) strings_wide_kernel(const __
       uint32_t total = tx;
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
-      if (lane == 0) {
-        h->r0     = r0;
+      if (lane == 0 && q == 0) {
         h->rows   = rows;
         h->direct = direct ? 1 : 0;
       }
       __syncwarp();
       if (lane == 0) {
-        if (total) mbar_arrive_expect_tx(&full[s], total);  // release: header / rowsm / hand copies visible
+        // release: header / rowsm / hand copies visible.  A producer none of whose rows carries bytes (null or empty
+        // strings, a short last tile) arrives without a transaction count.
+        if (total) mbar_arrive_expect_tx(&full[s], total);
         else mbar_arrive(&full[s]);
       }
       __syncwarp();
@@ -541,34 +560,45 @@ __global__ void __launch_bounds__(kSwMaxThreads, 1) strings_wide_kernel(const __
     }
   } else {
     // =================================== consumers ===================================
-    const int cw         = warp_id() - 1;
+    const int cw         = warp_id() - kSwProducers;
     const int gi         = cw / wpt;        // tile group
     const int wi         = cw - gi * wpt;   // warp inside the group
     const int c0         = wi * p.cpw;
     const int ncol       = tmax(0, tmin(p.nstr, c0 + p.cpw) - c0);
     const uint32_t stg_s = smem_u32(stg0 + static_cast<size_t>(cw) * kSwLine);
     const bool semi      = p.bases != nullptr;  // offsets hold group-local sums: finish them here
+    // this warp's columns at the group's iteration it_ (tile blockIdx.x + it_ * gridDim.x): b = the chars of column
+    // c0 + lane before the tile, vv[j] = the offsets entry of column c0 + j after the lane's row
+    auto load_cols = [&](int it_, int32_t& b, int32_t (&vv)[kSwMaxCpw]) {
+      const int64_t T = blockIdx.x + static_cast<int64_t>(it_) * gridDim.x;
+      const int64_t r = T << 5;
+      b               = 0;
+#pragma unroll
+      for (int j = 0; j < kSwMaxCpw; ++j) vv[j] = 0;
+      if (T >= ntiles) return;
+      if (lane < ncol) b = semi ? static_cast<int32_t>(p.bases[static_cast<int64_t>(c0 + lane) * ntiles + T]) : ldg_s32(s_offs[c0 + lane] + r);
+      const bool act = r + lane < p.num_rows;
+#pragma unroll
+      for (int j = 0; j < kSwMaxCpw; ++j)
+        if (j < ncol && act) vv[j] = ldg_s32(s_offs[c0 + j] + r + 1 + lane);
+    };
+    int32_t base_l, v[kSwMaxCpw];  // this tile's, loaded one tile ahead
+    load_cols(gi, base_l, v);
     for (int it = gi, k = 0;; it += kSwNG, ++k) {
       const int s        = it % NS;
       const uint32_t par = (it / NS) & 1;
+      int32_t nbase, nv[kSwMaxCpw];
+      load_cols(it + kSwNG, nbase, nv);  // the group's next tile: in flight during the wait and this tile's work
       mbar_wait(&full[s], par);
       const SwHdr h = hdr0[s];
       if (h.rows == 0) break;
+      const int64_t r0    = (blockIdx.x + static_cast<int64_t>(it) * gridDim.x) << 5;
       const int rows      = h.rows;
       const int last      = rows - 1;
       const bool active   = lane < rows;
       const bool direct   = h.direct != 0;
       const uint32_t pay_s = smem_u32(payload0 + static_cast<size_t>(s) * stage_span + kSwFront);
       // ---- this warp's columns: offsets entries of the tile -> lengths ------------------------------------
-      int32_t base_l = 0;  // chars of column c0 + lane before this tile
-      if (lane < ncol)
-        base_l = semi ? static_cast<int32_t>(p.bases[static_cast<int64_t>(c0 + lane) * ntiles + (h.r0 >> 5)]) : ldg_s32(s_offs[c0 + lane] + h.r0);
-      int32_t v[kSwMaxCpw];
-#pragma unroll
-      for (int j = 0; j < kSwMaxCpw; ++j) {
-        v[j] = 0;
-        if (j < ncol && active) v[j] = ldg_s32(s_offs[c0 + j] + h.r0 + 1 + lane);
-      }
       int32_t inc[kSwMaxCpw], len[kSwMaxCpw];
       int32_t mysum = 0;
 #pragma unroll
@@ -594,7 +624,7 @@ __global__ void __launch_bounds__(kSwMaxThreads, 1) strings_wide_kernel(const __
         var_s = pay_s + static_cast<uint32_t>(active ? rowsm0[s * 32 + lane] : 0);
       } else {
         var_g = reinterpret_cast<uint64_t>(p.rows) +
-                (active ? static_cast<uint64_t>(static_cast<uint32_t>(p.row_offsets[h.r0 + lane])) + p.size_per_row : 0);
+                (active ? static_cast<uint64_t>(static_cast<uint32_t>(p.row_offsets[r0 + lane])) + p.size_per_row : 0);
       }
 #pragma unroll
       for (int j = 0; j < kSwMaxCpw; ++j) {
@@ -606,8 +636,8 @@ __global__ void __launch_bounds__(kSwMaxThreads, 1) strings_wide_kernel(const __
           const int32_t rb = run;
           run += L;
           if (semi) {  // finish the offsets: one coalesced 128-byte store per column
-            if (active) asm volatile("st.global.s32 [%0], %1;" ::"l"(s_offs[c0 + j] + h.r0 + 1 + lane), "r"(bj + inc[j]));
-            if (h.r0 == 0 && lane == 0) asm volatile("st.global.s32 [%0], %1;" ::"l"(s_offs[c0 + j]), "r"(0));
+            if (active) asm volatile("st.global.s32 [%0], %1;" ::"l"(s_offs[c0 + j] + r0 + 1 + lane), "r"(bj + inc[j]));
+            if (r0 == 0 && lane == 0) asm volatile("st.global.s32 [%0], %1;" ::"l"(s_offs[c0 + j]), "r"(0));
           }
           if (T > 0) {
             uint8_t* D     = s_chars[c0 + j] + bj;
@@ -629,6 +659,9 @@ __global__ void __launch_bounds__(kSwMaxThreads, 1) strings_wide_kernel(const __
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty[s]);
+      base_l = nbase;
+#pragma unroll
+      for (int j = 0; j < kSwMaxCpw; ++j) v[j] = nv[j];
     }
   }
 }
@@ -697,7 +730,7 @@ int launch_strings_from_rows(const srj_plan* plan, const uint8_t* rows, const in
     const int64_t grid      = std::min<int64_t>(nsm, ntiles);
     const size_t smem       = strings_wide_smem_bytes(nstr, p.stage_bytes, p.wpt);
     SRJ_CUDA_TRY(cudaFuncSetAttribute(strings_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
-    strings_wide_kernel<<<static_cast<unsigned>(grid), (1 + kSwNG * p.wpt) * 32, smem, stream>>>(p);
+    strings_wide_kernel<<<static_cast<unsigned>(grid), (kSwProducers + kSwNG * p.wpt) * 32, smem, stream>>>(p);
     SRJ_CUDA_TRY(cudaGetLastError());
     return SRJ_OK;
   }
