@@ -284,6 +284,31 @@ SRJ_API int64_t srj_bloom_filter_merge_workspace_bytes(void);
 SRJ_API int srj_bloom_filter_merge(const uint8_t* filters, int64_t filters_bytes, int32_t num_filters, uint8_t* out, void* workspace,
                                    void* stream);
 
+/* ---- ZOrder.interleaveBits / hilbertIndex, ZOrder.java:29-87, zorder.cu:137-267 --------------------------------------
+ * Both read a row's N values MSB first, column-interleaved: stream position i holds bit B - 1 - i / N of column i % N,
+ * where a value is its little-endian bytes as an unsigned B-bit integer (two's complement, raw IEEE bits) and a null row
+ * counts as 0.
+ *   srj_interleave_bits_sizes : (host only, no device) *total_bytes = num_rows * N * W.  Checks every argument of
+ *                               srj_interleave_bits: N >= 1 columns of num_rows rows each, one fixed-width type id for all
+ *                               of them (DECIMAL scales are not compared); W is its size.  SRJ_EUNSUPPORTED for a type that
+ *                               is not fixed-width, SRJ_EINVAL for the rest, including num_rows * N * W > INT32_MAX.
+ *   srj_interleave_bits       : (async) Delta Lake's InterleaveBits, B = 8W: row r is the N * W bytes
+ *                               out_bytes[r * N * W ..) holding the stream (byte 0 = positions 0..7, MSB first), and
+ *                               out_offsets[0 .. num_rows] = r * N * W: the offsets and chars of a LIST<UINT8> column
+ *                               with no null mask.
+ *   srj_hilbert_index         : (async) out[r] = the Hilbert index of the point (X[0] .. X[N-1]) of row r, B = num_bits,
+ *                               X[c] = the INT32 value's low num_bits bits: Skilling's AxesToTranspose with Gray encoding
+ *                               (AIP Conf. Proc. 707, 2004), then the stream of the transposed coordinates read as an
+ *                               N * num_bits-bit integer.  SRJ_EINVAL for num_bits outside [1, 32], num_bits * N > 64,
+ *                               N < 1 or a row count that differs; SRJ_EUNSUPPORTED for a column that is not INT32.
+ * Inputs need element alignment (8 bytes for DECIMAL128); the outputs may be unaligned.  No synchronisation.
+ */
+SRJ_API int srj_interleave_bits_sizes(const srj_column* cols, int32_t num_columns, int64_t num_rows, int64_t* total_bytes);
+SRJ_API int srj_interleave_bits(const srj_column* cols, int32_t num_columns, int64_t num_rows, int32_t* out_offsets, uint8_t* out_bytes,
+                                void* stream);
+SRJ_API int srj_hilbert_index(int32_t num_bits, const srj_column* cols, int32_t num_columns, int64_t num_rows, int64_t* out,
+                              void* stream);
+
 /* ---- multi-GPU configuration (SURVEY 8e: row-range shards + one all-gather of per-column chunks) ---------------- */
 /* ---- Spark HashPartitioning on the device (SURVEY 8f rank 1) ---------------------------------------------------
  * The consumer of Hash.murmurHash32: GpuHashPartitioning computes pmod(murmur3_32(42, keys), P) per row and then

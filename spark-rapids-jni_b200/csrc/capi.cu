@@ -875,6 +875,80 @@ int srj_bloom_filter_merge(const uint8_t* filters, int64_t filters_bytes, int32_
 }
 
 // ---------------------------------------------------------------------------------------------------
+// ZOrder: interleaveBits and hilbertIndex (zorder.cu)
+// ---------------------------------------------------------------------------------------------------
+// zorder.cu:141-159: at least one column, fixed-width, one type id, the output within INT32_MAX bytes (a logic_error in
+// the reference, so SRJ_EINVAL rather than SRJ_EOVERFLOW).  *elem_bytes = W.
+static int interleave_check(const char* what, const srj_column* cols, int32_t n, int64_t rows, int32_t* elem_bytes)
+{
+  if (n <= 0 || !cols) { set_error("%s: The input table must have at least one column.", what); return SRJ_EINVAL; }
+  if (rows < 0) { set_error("%s: bad row count", what); return SRJ_EINVAL; }
+  const int32_t w = size_of_type(cols[0].type_id);
+  if (w == 0) { set_error("%s: Only fixed width columns can be used (type id %d)", what, cols[0].type_id); return SRJ_EUNSUPPORTED; }
+  for (int32_t c = 0; c < n; ++c) {
+    if (cols[c].type_id != cols[0].type_id) { set_error("%s: All columns of the input table must be the same type.", what); return SRJ_EINVAL; }
+    if (cols[c].size != rows) { set_error("%s: column %d has %lld rows, expected %lld", what, c, static_cast<long long>(cols[c].size), static_cast<long long>(rows)); return SRJ_EINVAL; }
+  }
+  if (rows * static_cast<int64_t>(w) * n > INT32_MAX) { set_error("%s: Input is too large to process", what); return SRJ_EINVAL; }
+  *elem_bytes = w;
+  return SRJ_OK;
+}
+
+// the data of every column present and aligned to its element (8 bytes for DECIMAL128: it is loaded as two longs)
+static int zorder_check_data(const char* what, const srj_column* cols, int32_t n, int64_t rows, int32_t w)
+{
+  if (rows == 0) return SRJ_OK;
+  const uintptr_t align = static_cast<uintptr_t>(w < 8 ? w : 8);
+  for (int32_t c = 0; c < n; ++c)
+    if (!cols[c].data || (reinterpret_cast<uintptr_t>(cols[c].data) & (align - 1))) {
+      set_error("%s: column %d has no data or data not aligned to %d bytes", what, c, static_cast<int>(align));
+      return SRJ_EINVAL;
+    }
+  return SRJ_OK;
+}
+
+int srj_interleave_bits_sizes(const srj_column* cols, int32_t num_columns, int64_t num_rows, int64_t* total_bytes)
+{
+  SRJ_API_RANGE();
+  if (!total_bytes) { set_error("interleave_bits_sizes: bad argument"); return SRJ_EINVAL; }
+  int32_t w    = 0;
+  const int rc = interleave_check("interleave_bits_sizes", cols, num_columns, num_rows, &w);
+  if (rc != SRJ_OK) return rc;
+  *total_bytes = num_rows * w * num_columns;
+  return SRJ_OK;
+}
+
+int srj_interleave_bits(const srj_column* cols, int32_t num_columns, int64_t num_rows, int32_t* out_offsets, uint8_t* out_bytes, void* stream)
+{
+  SRJ_API_RANGE();
+  int32_t w = 0;
+  int rc    = interleave_check("interleave_bits", cols, num_columns, num_rows, &w);
+  if (rc != SRJ_OK) return rc;
+  if ((rc = zorder_check_data("interleave_bits", cols, num_columns, num_rows, w)) != SRJ_OK) return rc;
+  if (!out_offsets || (num_rows > 0 && !out_bytes)) { set_error("interleave_bits: the output offsets and bytes are needed"); return SRJ_EINVAL; }
+  return launch_interleave_bits(cols, num_columns, num_rows, w, out_offsets, out_bytes, static_cast<cudaStream_t>(stream));
+}
+
+// zorder.cu:226-237
+int srj_hilbert_index(int32_t num_bits, const srj_column* cols, int32_t num_columns, int64_t num_rows, int64_t* out, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "hilbert_index";
+  if (num_bits <= 0 || num_bits > 32) { set_error("%s: the number of bits must be >0 and <= 32.", what); return SRJ_EINVAL; }
+  if (static_cast<int64_t>(num_bits) * num_columns > 64) { set_error("%s: we only support up to 64 bits of output right now.", what); return SRJ_EINVAL; }
+  if (num_columns <= 0 || !cols) { set_error("%s: at least one column is required.", what); return SRJ_EINVAL; }
+  if (num_rows < 0) { set_error("%s: bad row count", what); return SRJ_EINVAL; }
+  for (int32_t c = 0; c < num_columns; ++c) {
+    if (cols[c].type_id != SRJ_INT32) { set_error("%s: All columns of the input table must be INT32.", what); return SRJ_EUNSUPPORTED; }
+    if (cols[c].size != num_rows) { set_error("%s: column %d has %lld rows, expected %lld", what, c, static_cast<long long>(cols[c].size), static_cast<long long>(num_rows)); return SRJ_EINVAL; }
+  }
+  const int rc = zorder_check_data(what, cols, num_columns, num_rows, 4);
+  if (rc != SRJ_OK) return rc;
+  if (num_rows > 0 && !out) { set_error("%s: the output is null", what); return SRJ_EINVAL; }
+  return launch_hilbert_index(num_bits, cols, num_columns, num_rows, out, static_cast<cudaStream_t>(stream));
+}
+
+// ---------------------------------------------------------------------------------------------------
 // Spark HashPartitioning: pmod(murmur3_32(seed, keys), P) + stable partition (partition.cu)
 // ---------------------------------------------------------------------------------------------------
 int64_t srj_partition_workspace_bytes(int64_t num_rows, int32_t num_partitions)

@@ -118,6 +118,12 @@ int launch_bloom_probe(const BloomHeader& h, const uint8_t* buf, const srj_colum
 // header copy, header check (*d_flag <- 1 on a mismatch) and the word-wise OR of `nfilters` filters `stride` bytes apart
 int launch_bloom_merge(const uint8_t* child, int64_t stride, int32_t nfilters, int hdr_bytes, uint8_t* out, int32_t* d_flag, cudaStream_t stream);
 
+// ---- zorder.cu: ZOrder.interleaveBits / hilbertIndex (the caller has checked every argument) ----
+// out_offsets: rows + 1 int32 (r * ncols * elem_bytes); out: rows * ncols * elem_bytes bytes.  Either may be unaligned.
+int launch_interleave_bits(const srj_column* cols, int32_t ncols, int64_t rows, int32_t elem_bytes, int32_t* out_offsets, uint8_t* out,
+                           cudaStream_t stream);
+int launch_hilbert_index(int32_t num_bits, const srj_column* cols, int32_t ncols, int64_t rows, int64_t* out, cudaStream_t stream);
+
 // ---- kudo.cu: the Kudo shuffle wire format for flat tables (split / assemble) ----
 int64_t kudo_workspace_bytes(int32_t ncols, int32_t P);
 int launch_kudo_split_sizes(const srj_column* cols, int32_t ncols, int64_t num_rows, const int32_t* d_splits, int32_t P, int64_t* d_part_offsets,
