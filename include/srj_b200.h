@@ -309,6 +309,45 @@ SRJ_API int srj_interleave_bits(const srj_column* cols, int32_t num_columns, int
 SRJ_API int srj_hilbert_index(int32_t num_bits, const srj_column* cols, int32_t num_columns, int64_t num_rows, int64_t* out,
                               void* stream);
 
+/* ---- Iceberg partition transforms: IcebergBucket / IcebergTruncate / IcebergDateTimeUtil ------------------------------
+ * Reference iceberg/iceberg_bucket.cu:388-457, iceberg_truncate.cu:141-238, iceberg_datetime_util.cu:137-248.  Every
+ * result has the input's rows; out_mask (ceil(rows / 32) words) receives a copy of the input's null mask (all ones when
+ * the input has none) and may be NULL only when the input has no mask.  The null count is the input's.
+ *   srj_iceberg_bucket       : (async) out[r] = (murmur3_x86_32(bytes, 0) & INT32_MAX) % num_buckets, 0 for a null row.
+ *                              Bytes: INT32 / TIMESTAMP_DAYS widened to int64, INT64 / TIMESTAMP_MICROSECONDS: 8 bytes
+ *                              little-endian; DECIMAL32/64/128: BigInteger.toByteArray() of the unscaled value; STRING:
+ *                              the chars; LIST<UINT8>: the child bytes.  SRJ_EINVAL for num_buckets <= 0,
+ *                              SRJ_EUNSUPPORTED for another type or a LIST whose child is not UINT8.
+ *   srj_iceberg_truncate_workspace_bytes : bytes of srj_iceberg_truncate_sizes' workspace.
+ *   srj_iceberg_truncate_sizes : STRING / LIST<UINT8> only: d_out_offsets[0 .. rows] of the output and *total_bytes (host;
+ *                              synchronises the stream once).  A null row has zero length.  STRING keeps the bytes before
+ *                              the (width+1)-th byte that is not a UTF-8 continuation byte (all of them when there is
+ *                              none); LIST<UINT8> keeps min(len, width) bytes.
+ *   srj_iceberg_truncate     : (async) INT32, INT64, DECIMAL32/64/128: out->data[r] = v - (((v % W) + W) % W) in the
+ *                              storage type (W = width sign-extended, % truncated, + and - wrapping), 0 for a null row.
+ *                              STRING: out->offsets (from the sizes call) and the chars in out->data; LIST<UINT8>:
+ *                              out->offsets and the bytes in out->children[0].data.  SRJ_EINVAL for width == 0
+ *                              (integral) or width <= 0 (STRING / LIST) and for a LIST child with a null mask;
+ *                              SRJ_EUNSUPPORTED for another type.
+ *   srj_iceberg_datetime     : (async) transform SRJ_ICEBERG_YEARS / MONTHS / DAYS / HOURS of a TIMESTAMP_DAYS (not
+ *                              HOURS) or TIMESTAMP_MICROSECONDS column: years and months since 1970-01 (proleptic
+ *                              Gregorian), days since 1970-01-01, hours since the epoch (wrapping to int32), from the
+ *                              floored day / hour.  out is int32 per row (TIMESTAMP_DAYS for DAYS).  Rows under nulls are
+ *                              computed from their bits.  SRJ_EINVAL for an unknown transform, SRJ_EUNSUPPORTED for
+ *                              another type.
+ * Fixed-width inputs and outputs need element alignment (8 bytes for DECIMAL128); offsets need 4 bytes.
+ */
+#define SRJ_ICEBERG_YEARS 0
+#define SRJ_ICEBERG_MONTHS 1
+#define SRJ_ICEBERG_DAYS 2
+#define SRJ_ICEBERG_HOURS 3
+SRJ_API int srj_iceberg_bucket(const srj_column* input, int32_t num_buckets, int32_t* out, uint32_t* out_mask, void* stream);
+SRJ_API int64_t srj_iceberg_truncate_workspace_bytes(int64_t num_rows);
+SRJ_API int srj_iceberg_truncate_sizes(const srj_column* input, int32_t width, int32_t* d_out_offsets, int64_t* total_bytes,
+                                       void* workspace, void* stream);
+SRJ_API int srj_iceberg_truncate(const srj_column* input, int32_t width, const srj_column* out, void* stream);
+SRJ_API int srj_iceberg_datetime(int32_t transform, const srj_column* input, int32_t* out, uint32_t* out_mask, void* stream);
+
 /* ---- multi-GPU configuration (SURVEY 8e: row-range shards + one all-gather of per-column chunks) ---------------- */
 /* ---- Spark HashPartitioning on the device (SURVEY 8f rank 1) ---------------------------------------------------
  * The consumer of Hash.murmurHash32: GpuHashPartitioning computes pmod(murmur3_32(42, keys), P) per row and then

@@ -12,13 +12,12 @@
 //   V1: for i = 1..k:  c = (int32)(h1 + i * h2),  p = (c < 0 ? ~c : c) % bits
 //   V2: c = (int64)h1 * INT32_MAX;  for i = 0..k-1:  c += (int64)h2,  p = (c < 0 ? ~c : c) % bits
 //
-// The modulo by the per-call constant `bits` uses a host-computed reciprocal m = floor((2^N - 1) / bits) (N = 32 for
-// V1's 31-bit dividends, 64 for V2's 63-bit ones): q = mulhi(x, m) is floor(x / bits) or one less (x < 2^(N-1) keeps
-// the error under 3/2), so r = x - q * bits needs at most one conditional subtraction.  No division instruction or
-// subroutine is left in the put / probe loops.
+// The modulo by the per-call constant `bits` uses a host-computed reciprocal (reciprocal.cuh: mod_v1 for V1's 31-bit
+// dividends, mod_v2 for V2's 63-bit ones).  No division instruction or subroutine is left in the put / probe loops.
 #include "common.cuh"
 #include "hash_device.cuh"
 #include "kernels.hpp"
+#include "reciprocal.cuh"
 
 namespace srj {
 namespace {
@@ -26,18 +25,6 @@ namespace {
 constexpr int kBloomThreads = 256;
 constexpr int kRowsPerThread = 4;   // 2 x 16-byte key loads in, one 4-byte BOOL8 store out
 constexpr int kHashChunk     = 8;   // word loads of one row issued together before any is tested
-
-__device__ __forceinline__ uint32_t mod_v1(uint32_t x, uint32_t d, uint32_t m)
-{
-  uint32_t r = x - __umulhi(x, m) * d;
-  return r >= d ? r - d : r;
-}
-
-__device__ __forceinline__ uint64_t mod_v2(uint64_t x, uint64_t d, uint64_t m)
-{
-  uint64_t r = x - __umul64hi(x, m) * d;
-  return r >= d ? r - d : r;
-}
 
 // The k bit positions of one key, produced one at a time (V1 state in 32 bits, V2 in 64).
 template <int V>
@@ -212,7 +199,7 @@ unsigned grid_for(int64_t threads) { return static_cast<unsigned>((threads + kBl
 
 uint64_t bloom_reciprocal(int32_t version, uint64_t bits)
 {
-  return version == 1 ? static_cast<uint64_t>(0xffffffffu / static_cast<uint32_t>(bits)) : ~uint64_t{0} / bits;
+  return version == 1 ? reciprocal_v1(static_cast<uint32_t>(bits)) : reciprocal_v2(bits);
 }
 
 int launch_bloom_init(const BloomHeader& h, uint8_t* buf, cudaStream_t stream)

@@ -130,6 +130,16 @@ __device__ inline uint32_t mm_bytes(const uint8_t* d, int32_t len, uint32_t seed
     h = mm_mix(h, static_cast<uint32_t>(static_cast<int32_t>(static_cast<int8_t>(d[i]))));  // murmur_hash.cuh:72-93
   return mm_fmix(h, static_cast<uint32_t>(len));
 }
+// Standard MurmurHash3_x86_32 (Iceberg's bucket hash, Guava's murmur3_32): the 4-byte blocks are mm_mix, but the 1-3 tail
+// bytes are folded into one little-endian word k1 (upper bytes zero), scrambled and XORed into h without the
+// rotate-multiply-add of a block.  iceberg.cu feeds the blocks and that tail word from registers.
+__device__ __forceinline__ uint32_t mm_tail_std(uint32_t h, uint32_t k1)
+{
+  k1 *= MC1;
+  k1 = __funnelshift_l(k1, k1, 15);
+  k1 *= MC2;
+  return h ^ k1;
+}
 
 // ---------------------------------------------------------------- float canonicalisation (hash.cuh:34-57)
 __device__ __forceinline__ uint32_t norm_f32(uint32_t bits, bool zeros)

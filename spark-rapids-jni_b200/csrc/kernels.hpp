@@ -124,6 +124,17 @@ int launch_interleave_bits(const srj_column* cols, int32_t ncols, int64_t rows, 
                            cudaStream_t stream);
 int launch_hilbert_index(int32_t num_bits, const srj_column* cols, int32_t ncols, int64_t rows, int64_t* out, cudaStream_t stream);
 
+// ---- iceberg.cu: Iceberg's bucket / truncate / date-time transforms (the caller has checked every argument) ----
+// out_mask (NULL: none) gets a copy of the input's mask, all ones when the input has none.
+int launch_iceberg_bucket(const srj_column& in, int32_t num_buckets, int32_t* out, uint32_t* out_mask, cudaStream_t stream);
+int launch_iceberg_truncate_fixed(const srj_column& in, int32_t width, void* out, uint32_t* out_mask, cudaStream_t stream);
+int64_t iceberg_truncate_workspace_bytes(int64_t n);
+// STRING / LIST<UINT8>: d_offsets[0 .. n] and *h_total (reads the total back: one stream synchronisation)
+int launch_iceberg_truncate_sizes(const srj_column& in, int32_t width, int32_t* d_offsets, int64_t* h_total, void* workspace,
+                                  cudaStream_t stream);
+int launch_iceberg_truncate_bytes(const srj_column& in, const int32_t* out_offsets, uint8_t* out_bytes, uint32_t* out_mask, cudaStream_t stream);
+int launch_iceberg_datetime(int32_t transform, const srj_column& in, int32_t* out, uint32_t* out_mask, cudaStream_t stream);
+
 // ---- kudo.cu: the Kudo shuffle wire format for flat tables (split / assemble) ----
 int64_t kudo_workspace_bytes(int32_t ncols, int32_t P);
 int launch_kudo_split_sizes(const srj_column* cols, int32_t ncols, int64_t num_rows, const int32_t* d_splits, int32_t P, int64_t* d_part_offsets,

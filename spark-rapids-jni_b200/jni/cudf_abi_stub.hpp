@@ -22,7 +22,8 @@ struct device_buffer {
 namespace cudf {
 using size_type     = int32_t;
 using bitmask_type  = uint32_t;
-enum class type_id : int32_t { EMPTY = 0, INT8 = 1, UINT8 = 5, INT32 = 3, INT64 = 4, BOOL8 = 11, STRING = 23, LIST = 24 };
+enum class type_id : int32_t { EMPTY = 0, INT8 = 1, UINT8 = 5, INT32 = 3, INT64 = 4, BOOL8 = 11, TIMESTAMP_DAYS = 12, TIMESTAMP_MICROSECONDS = 15,
+                              STRING = 23, LIST = 24, DECIMAL32 = 25, DECIMAL64 = 26, DECIMAL128 = 27 };
 struct data_type {
   data_type(type_id id, int32_t scale = 0);
   type_id id() const;
@@ -56,6 +57,7 @@ struct column {
 };
 struct lists_column_view {                           // lists/lists_column_view.hpp
   explicit lists_column_view(column_view const& lists);
+  column_view offsets() const;
   column_view child() const;
   size_type size() const;
 };

@@ -9,6 +9,7 @@
 #include <cudf/column/column.hpp>
 #include <cudf/column/column_factories.hpp>
 #include <cudf/column/column_view.hpp>
+#include <cudf/lists/lists_column_view.hpp>
 #include <cudf/table/table_view.hpp>
 #include <cudf/utilities/default_stream.hpp>
 #include <rmm/device_buffer.hpp>
@@ -91,6 +92,29 @@ inline srj_column to_srj(const cudf::column_view& c)
     s.data = const_cast<uint8_t*>(c.head<uint8_t>());
   }
   return s;
+}
+
+// to_srj for any input of the Iceberg transforms: a LIST<UINT8> (binary) column also gets its offsets and its element
+// column, described in *child (which must outlive the returned descriptor's use)
+inline srj_column to_srj_any(const cudf::column_view& c, srj_column* child)
+{
+  if (c.type().id() != cudf::type_id::LIST) return to_srj(c);
+  srj_column s{};
+  s.type_id   = SRJ_LIST;
+  s.size      = c.size();
+  s.null_mask = const_cast<uint32_t*>(c.null_mask());
+  cudf::lists_column_view const lists(c);
+  s.offsets          = const_cast<int32_t*>(lists.offsets().head<int32_t>());
+  *child             = to_srj(lists.child());
+  s.children         = child;
+  s.num_children     = 1;
+  return s;
+}
+
+// a device buffer for a copy of the input's null mask (empty when the input has none)
+inline rmm::device_buffer mask_like(const srj_column& in, rmm::cuda_stream_view stream)
+{
+  return rmm::device_buffer(in.null_mask ? static_cast<size_t>((in.size + 31) / 32) * 4 : 0, stream);
 }
 
 inline int32_t size_of_type(int32_t t)
