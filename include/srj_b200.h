@@ -348,6 +348,37 @@ SRJ_API int srj_iceberg_truncate_sizes(const srj_column* input, int32_t width, i
 SRJ_API int srj_iceberg_truncate(const srj_column* input, int32_t width, const srj_column* out, void* stream);
 SRJ_API int srj_iceberg_datetime(int32_t transform, const srj_column* input, int32_t* out, uint32_t* out_mask, void* stream);
 
+/* ---- DecimalUtils: DECIMAL128 multiply, divide, integral divide, remainder, add and subtract -------------------------
+ * Reference decimal_utils.cu:529-1167 (multiply_decimal128 .. sub_decimal128).  a and b are DECIMAL128 columns with the
+ * same row count; a value is v * 10^scale (cudf scale).  Every row, null or not, is computed from the bits under it in
+ * 256-bit two's complement, as the reference does:
+ *   SRJ_DECIMAL_MULTIPLY       : a * b rounded HALF_UP to out_scale; with interim_cast, first rounded to 38 digits when
+ *                                it has more (Spark's SPARK-40129 behaviour).  A row whose scale-up would pass 38 digits
+ *                                overflows with value 0.
+ *   SRJ_DECIMAL_DIVIDE         : a / b rounded HALF_UP to out_scale.
+ *   SRJ_DECIMAL_INTEGER_DIVIDE : a / b truncated at out_scale (0 for Spark's div); out is int64 per row, the low 64 bits
+ *                                of the quotient, whose overflow flag is judged on the whole quotient.
+ *   SRJ_DECIMAL_REMAINDER      : a - (a div b) * b at out_scale, with the sign of a (Java's BigDecimal.remainder).
+ *   SRJ_DECIMAL_ADD / SUBTRACT : a + b or a - b at min(a.scale, b.scale), then rounded HALF_UP to out_scale.
+ * overflow[r] (BOOL8) is 1 when |result| >= 10^38 or b is 0 (divide family; value 0).  out holds 16 bytes per row (8 for
+ * INTEGER_DIVIDE): the low bits of the result.  When a or b has a null mask, out_mask (ceil(rows / 32) words) receives the
+ * AND of the masks and *null_count its null count, read back with one stream synchronisation; otherwise *null_count (if
+ * given) is 0, out_mask is not written and the call is asynchronous.  Both output columns take that mask.
+ * SRJ_EUNSUPPORTED when a or b is not DECIMAL128; SRJ_EINVAL for an unknown op, differing row counts, a missing buffer,
+ * and for the scale combinations whose rows would need a power of ten the reference cannot represent (multiply:
+ * out_scale - (a.scale + b.scale) > 38; divide: out_scale - (a.scale - b.scale) outside [-114, 38]; remainder: a divisor
+ * or dividend shift above 38 or below -76; add / subtract: |a.scale - b.scale| > 76, or out_scale more than 38 above or
+ * 76 below min(a.scale, b.scale)).  Inputs need 8-byte alignment, out 8 bytes, out_mask 4; overflow may be unaligned.
+ */
+#define SRJ_DECIMAL_MULTIPLY 0
+#define SRJ_DECIMAL_DIVIDE 1
+#define SRJ_DECIMAL_INTEGER_DIVIDE 2
+#define SRJ_DECIMAL_REMAINDER 3
+#define SRJ_DECIMAL_ADD 4
+#define SRJ_DECIMAL_SUBTRACT 5
+SRJ_API int srj_decimal128_binary(int32_t op, const srj_column* a, const srj_column* b, int32_t out_scale, int32_t interim_cast,
+                                  uint8_t* overflow, void* out, uint32_t* out_mask, int64_t* null_count, void* stream);
+
 /* ---- multi-GPU configuration (SURVEY 8e: row-range shards + one all-gather of per-column chunks) ---------------- */
 /* ---- Spark HashPartitioning on the device (SURVEY 8f rank 1) ---------------------------------------------------
  * The consumer of Hash.murmurHash32: GpuHashPartitioning computes pmod(murmur3_32(42, keys), P) per row and then

@@ -135,6 +135,12 @@ int launch_iceberg_truncate_sizes(const srj_column& in, int32_t width, int32_t* 
 int launch_iceberg_truncate_bytes(const srj_column& in, const int32_t* out_offsets, uint8_t* out_bytes, uint32_t* out_mask, cudaStream_t stream);
 int launch_iceberg_datetime(int32_t transform, const srj_column& in, int32_t* out, uint32_t* out_mask, cudaStream_t stream);
 
+// ---- decimal.cu: DecimalUtils' DECIMAL128 arithmetic (the caller has checked every argument and scale) ----
+// Writes out_mask (the AND of the input masks) and *null_count when an input has a mask, reading the count back (one
+// stream synchronisation); otherwise *null_count = 0 and out_mask is untouched.
+int launch_decimal128_binary(int32_t op, const srj_column& a, const srj_column& b, int32_t out_scale, bool interim_cast, uint8_t* ovf,
+                             void* out, uint32_t* out_mask, int64_t* null_count, cudaStream_t stream);
+
 // ---- kudo.cu: the Kudo shuffle wire format for flat tables (split / assemble) ----
 int64_t kudo_workspace_bytes(int32_t ncols, int32_t P);
 int launch_kudo_split_sizes(const srj_column* cols, int32_t ncols, int64_t num_rows, const int32_t* d_splits, int32_t P, int64_t* d_part_offsets,

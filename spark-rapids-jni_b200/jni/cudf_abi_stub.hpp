@@ -14,6 +14,7 @@ struct cuda_stream_view { void* value() const; void synchronize() const; };
 struct device_buffer {
   device_buffer();
   device_buffer(std::size_t bytes, cuda_stream_view stream);
+  device_buffer(void const* source, std::size_t bytes, cuda_stream_view stream);   // a device-to-device copy
   void* data();
   std::size_t size() const;
 };

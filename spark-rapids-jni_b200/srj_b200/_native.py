@@ -82,6 +82,8 @@ SYMBOLS = {
     "srj_iceberg_truncate_sizes": (C.c_int, [C.POINTER(SrjColumn), C.c_int32, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p, C.c_void_p]),
     "srj_iceberg_truncate": (C.c_int, [C.POINTER(SrjColumn), C.c_int32, C.POINTER(SrjColumn), C.c_void_p]),
     "srj_iceberg_datetime": (C.c_int, [C.c_int32, C.POINTER(SrjColumn), C.c_void_p, C.c_void_p, C.c_void_p]),
+    "srj_decimal128_binary": (C.c_int, [C.c_int32, C.POINTER(SrjColumn), C.POINTER(SrjColumn), C.c_int32, C.c_int32, C.c_void_p,
+                                        C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
     "srj_partition_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int32]),
     "srj_hash_partition": (C.c_int, [C.POINTER(SrjColumn), C.c_int32, C.c_int64, C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
