@@ -379,6 +379,40 @@ SRJ_API int srj_iceberg_datetime(int32_t transform, const srj_column* input, int
 SRJ_API int srj_decimal128_binary(int32_t op, const srj_column* a, const srj_column* b, int32_t out_scale, int32_t interim_cast,
                                   uint8_t* overflow, void* out, uint32_t* out_mask, int64_t* null_count, void* stream);
 
+/* ---- DateTimeUtils: Julian / Gregorian rebase and date / timestamp truncation ------------------------------------------
+ * Reference datetime_rebase.cu:342-372, datetime_truncate.cu:327-376.  Inputs are TIMESTAMP_DAYS (int32 days since
+ * 1970-01-01) or TIMESTAMP_MICROSECONDS (int64 microseconds since the epoch, UTC); out has the input's type.  Dates go
+ * through y/m/d with the year reduced to int16, as the reference's cuda::std::chrono::year does (DESIGN 3.6j).
+ *   srj_datetime_rebase   : (async) SRJ_DATETIME_GREGORIAN_TO_JULIAN: a day's proleptic Gregorian y/m/d read as a Julian
+ *                           date (1582-10-05 .. 14 -> 1582-10-15; from 1582-10-15 on unchanged); JULIAN_TO_GREGORIAN: the
+ *                           reverse (unchanged from day -141427 on).  Micros: unchanged from 1582-10-15T00:00Z on, else the
+ *                           floored day is rebased and the time of day reattached, wrapping in int64.  Rows under nulls
+ *                           are computed from their bits.  out_mask (ceil(rows / 32) words) receives a copy of the input's
+ *                           mask (all ones when it has none) and may be NULL only when the input has no mask; the null
+ *                           count is the input's.
+ *   srj_datetime_truncate : exactly one of format_col (a STRING column) and format (format_len bytes) is given.  Formats
+ *                           are ASCII case-insensitive: YEAR / YYYY / YY, QUARTER, MONTH / MM / MON, WEEK (the Monday on
+ *                           or before), and for TIMESTAMP_MICROSECONDS only DAY / DD, HOUR, MINUTE, SECOND, MILLISECOND,
+ *                           MICROSECOND (the time of day floored).  A row whose format is anything else is null.  Null
+ *                           rows hold 0.
+ *                           format: (async) rows = datetime rows.  A format that fits the type: out_mask receives a copy of
+ *                           the input's mask (may be NULL when it has none) and *null_count = -1, meaning the input's null
+ *                           count, which the caller holds.  Otherwise the result is all null: out and out_mask are zeroed
+ *                           (out_mask is needed) and *null_count = rows.
+ *                           format_col: rows = format rows; the datetime has one row, applied to every row, or as many as
+ *                           the format.  A row is null when its datetime, its format or the format's parse is.  out_mask is
+ *                           needed; *null_count is read back (one stream synchronisation).
+ *                           SRJ_EUNSUPPORTED for a datetime that is not a timestamp of days or microseconds or a format
+ *                           column that is not STRING; SRJ_EINVAL for other row counts or a missing null_count.
+ * Both: zero rows touch nothing.  SRJ_EINVAL for a missing or misaligned buffer (data and out at their element, offsets
+ * and out_mask at 4 bytes).
+ */
+#define SRJ_DATETIME_GREGORIAN_TO_JULIAN 0
+#define SRJ_DATETIME_JULIAN_TO_GREGORIAN 1
+SRJ_API int srj_datetime_rebase(int32_t direction, const srj_column* input, void* out, uint32_t* out_mask, void* stream);
+SRJ_API int srj_datetime_truncate(const srj_column* datetime, const srj_column* format_col, const char* format, int32_t format_len,
+                                  void* out, uint32_t* out_mask, int64_t* null_count, void* stream);
+
 /* ---- multi-GPU configuration (SURVEY 8e: row-range shards + one all-gather of per-column chunks) ---------------- */
 /* ---- Spark HashPartitioning on the device (SURVEY 8f rank 1) ---------------------------------------------------
  * The consumer of Hash.murmurHash32: GpuHashPartitioning computes pmod(murmur3_32(42, keys), P) per row and then

@@ -1132,6 +1132,79 @@ int srj_decimal128_binary(int32_t op, const srj_column* a, const srj_column* b, 
 }
 
 // ---------------------------------------------------------------------------------------------------
+// DateTimeUtils: calendar rebase and date / timestamp truncation (datetime.cu)
+// ---------------------------------------------------------------------------------------------------
+static bool is_datetime(int32_t t) { return t == SRJ_TIMESTAMP_DAYS || t == SRJ_TIMESTAMP_MICROSECONDS; }
+
+// rows > 0: the datetime data and out at the element's alignment
+static int datetime_check_data(const char* what, const srj_column* dt, const void* out)
+{
+  const int a = dt->type_id == SRJ_TIMESTAMP_DAYS ? 4 : 8;
+  if (!dt->data || !aligned_to(dt->data, a)) { set_error("%s: the datetime data is missing or not aligned to %d bytes", what, a); return SRJ_EINVAL; }
+  if (!out || !aligned_to(out, a)) { set_error("%s: the output is missing or not aligned to %d bytes", what, a); return SRJ_EINVAL; }
+  return SRJ_OK;
+}
+
+// datetime_rebase.cu:342-372
+int srj_datetime_rebase(int32_t direction, const srj_column* input, void* out, uint32_t* out_mask, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "datetime_rebase";
+  if (!input) { set_error("%s: bad argument", what); return SRJ_EINVAL; }
+  if (direction != SRJ_DATETIME_GREGORIAN_TO_JULIAN && direction != SRJ_DATETIME_JULIAN_TO_GREGORIAN) {
+    set_error("%s: unknown direction %d", what, direction);
+    return SRJ_EINVAL;
+  }
+  if (!is_datetime(input->type_id)) { set_error("%s: The input must be either day or microsecond timestamps to rebase.", what); return SRJ_EUNSUPPORTED; }
+  if (input->size < 0) { set_error("%s: bad row count", what); return SRJ_EINVAL; }
+  if (input->size == 0) return SRJ_OK;
+  const int rc = datetime_check_data(what, input, out);
+  if (rc != SRJ_OK) return rc;
+  if (input->null_mask && (!out_mask || !aligned_to(out_mask, 4))) { set_error("%s: the input has a null mask but no output mask was given", what); return SRJ_EINVAL; }
+  return launch_datetime_rebase(direction, *input, out, out_mask, static_cast<cudaStream_t>(stream));
+}
+
+// datetime_truncate.cu:327-376
+int srj_datetime_truncate(const srj_column* datetime, const srj_column* format_col, const char* format, int32_t format_len, void* out,
+                          uint32_t* out_mask, int64_t* null_count, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "datetime_truncate";
+  if (!datetime || !null_count || (format_col == nullptr) == (format == nullptr) || (format && format_len < 0)) {
+    set_error("%s: bad argument (give exactly one of a format column and a format string, and a null count)", what);
+    return SRJ_EINVAL;
+  }
+  if (!is_datetime(datetime->type_id)) { set_error("%s: The date/time input must be either day or microsecond timestamps.", what); return SRJ_EUNSUPPORTED; }
+  if (format_col && format_col->type_id != SRJ_STRING) { set_error("%s: The format input must be of string type.", what); return SRJ_EUNSUPPORTED; }
+  if (datetime->size < 0 || (format_col && format_col->size < 0)) { set_error("%s: bad row count", what); return SRJ_EINVAL; }
+  if (format_col && datetime->size != 1 && datetime->size != format_col->size) {
+    set_error("%s: The input date/time column must have exactly one row or the same number of rows as the format column.", what);
+    return SRJ_EINVAL;
+  }
+  const int64_t rows = format_col ? format_col->size : datetime->size;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (rows == 0) {
+    *null_count = 0;
+    return SRJ_OK;
+  }
+  const int rc = datetime_check_data(what, datetime, out);
+  if (rc != SRJ_OK) return rc;
+  if (format_col) {
+    if (!format_col->offsets || !aligned_to(format_col->offsets, 4)) { set_error("%s: the format offsets are missing or not 4-byte aligned", what); return SRJ_EINVAL; }
+    if (!out_mask || !aligned_to(out_mask, 4)) { set_error("%s: a format column needs an output mask", what); return SRJ_EINVAL; }
+    return launch_datetime_truncate_column(*datetime, *format_col, out, out_mask, null_count, s);
+  }
+  const int32_t fmt = datetime_parse_format(format, format_len);
+  const bool fits   = datetime_format_fits(fmt, datetime->type_id == SRJ_TIMESTAMP_MICROSECONDS);
+  if ((!fits || datetime->null_mask) && (!out_mask || !aligned_to(out_mask, 4))) {
+    set_error("%s: the result has nulls but no output mask was given", what);
+    return SRJ_EINVAL;
+  }
+  *null_count = fits ? -1 : rows;
+  return launch_datetime_truncate_scalar(fmt, *datetime, out, out_mask, s);
+}
+
+// ---------------------------------------------------------------------------------------------------
 // Spark HashPartitioning: pmod(murmur3_32(seed, keys), P) + stable partition (partition.cu)
 // ---------------------------------------------------------------------------------------------------
 int64_t srj_partition_workspace_bytes(int64_t num_rows, int32_t num_partitions)

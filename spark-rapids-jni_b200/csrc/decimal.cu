@@ -327,6 +327,11 @@ int launch(const srj_column& a, const srj_column& b, uint8_t* ovf, void* out, co
   return SRJ_OK;
 }
 
+U256 pow_or_one(int k) { return host_pow(k < 0 || k > kMaxPow ? 0 : k); }
+Div div_or_one(int k) { return host_div(k < 1 || k > 38 ? 0 : k); }
+
+}  // namespace
+
 // The null counter of the calling host thread on the current device, allocated once.  A call reads its count back before
 // it returns, and one host thread makes one call at a time, so a counter per (thread, device) is never shared by two calls
 // in flight.
@@ -352,11 +357,6 @@ int null_counter(unsigned long long** out)
   *out = p;
   return SRJ_OK;
 }
-
-U256 pow_or_one(int k) { return host_pow(k < 0 || k > kMaxPow ? 0 : k); }
-Div div_or_one(int k) { return host_div(k < 1 || k > 38 ? 0 : k); }
-
-}  // namespace
 
 int launch_decimal128_binary(int32_t op, const srj_column& a, const srj_column& b, int32_t out_scale, bool interim_cast, uint8_t* ovf,
                              void* out, uint32_t* out_mask, int64_t* null_count, cudaStream_t stream)

@@ -17,35 +17,29 @@
 // are loaded.
 #include <type_traits>
 
+#include "civil_date.cuh"
 #include "common.cuh"
 #include "hash_device.cuh"
 #include "kernels.hpp"
+#include "map_rows.cuh"
 #include "reciprocal.cuh"
 
 namespace srj {
 namespace {
 
 constexpr int kIceThreads = 256;
-constexpr int kIceRows    = 4;
+constexpr int kIceRows    = kMapRows;
 constexpr int kLaneCopy   = 16;   // truncate: rows of up to this many output bytes are copied by their own lane
 
 struct I128 {                     // DECIMAL128 storage: little-endian halves (8-byte alignment suffices)
   uint64_t lo, hi;
 };
 
-__device__ __forceinline__ int32_t ld_elem(const int32_t* p) { return __ldg(p); }
-__device__ __forceinline__ int64_t ld_elem(const int64_t* p) { return __ldg(reinterpret_cast<const long long*>(p)); }
 __device__ __forceinline__ I128 ld_elem(const I128* p)
 {
   const auto* q = reinterpret_cast<const unsigned long long*>(p);
   return I128{__ldg(q), __ldg(q + 1)};
 }
-
-template <class T>
-union RowBuf {
-  T v[kIceRows];
-  uint4 u[sizeof(T) * kIceRows / 16];
-};
 
 // ---- bucket ---------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t bswap32(uint64_t v) { return __byte_perm(static_cast<uint32_t>(v), 0, 0x0123); }   // of the low word
@@ -184,29 +178,6 @@ struct Trunc128 {
 };
 
 // ---- year / month / day / hour ----------------------------------------------------------------------------------------
-constexpr int64_t kMicrosPerDay  = 86400000000ll;
-constexpr int64_t kMicrosPerHour = 3600000000ll;
-
-template <int64_t D>
-__device__ __forceinline__ int64_t floor_div_const(int64_t t)
-{
-  const int64_t q = t / D;                    // by a constant: multiply-high, no division subroutine
-  return q - (t - q * D < 0);
-}
-
-// proleptic Gregorian year and month (1..12) of a day count from 1970-01-01 (Hinnant, civil_from_days)
-__device__ __forceinline__ void civil_year_month(int32_t days, int32_t* year, int32_t* month)
-{
-  const int64_t z    = static_cast<int64_t>(days) + 719468;               // days from 0000-03-01
-  const int64_t era  = (z >= 0 ? z : z - 146096) / 146097;
-  const uint32_t doe = static_cast<uint32_t>(z - era * 146097);           // [0, 146096]
-  const uint32_t yoe = (doe - doe / 1460 + doe / 36524 - doe / 146096) / 365;
-  const uint32_t doy = doe - (365 * yoe + yoe / 4 - yoe / 100);           // [0, 365], from March 1
-  const uint32_t mp  = (5 * doy + 2) / 153;                               // [0, 11], March = 0
-  *month             = static_cast<int32_t>(mp < 10 ? mp + 3 : mp - 9);
-  *year              = static_cast<int32_t>(yoe) + static_cast<int32_t>(era) * 400 + (*month <= 2);
-}
-
 template <int T, bool kMicros>   // T: SRJ_ICEBERG_YEARS / MONTHS / DAYS / HOURS
 struct DateOp {
   using In  = typename std::conditional<kMicros, int64_t, int32_t>::type;
@@ -229,51 +200,10 @@ template <class Op>
 __global__ void __launch_bounds__(kIceThreads) ice_map_kernel(const typename Op::In* __restrict__ in, const uint32_t* __restrict__ mask,
                                                               typename Op::Out* __restrict__ out, int64_t n, bool vec, const Op op)
 {
-  using In         = typename Op::In;
-  using Out        = typename Op::Out;
-  const int64_t r0 = (static_cast<int64_t>(blockIdx.x) * kIceThreads + threadIdx.x) * kIceRows;
-  if (r0 >= n) return;
-  const int cnt = static_cast<int>(tmin<int64_t>(kIceRows, n - r0));
-  RowBuf<In> a;
-  if (vec && cnt == kIceRows) {
-#pragma unroll
-    for (int i = 0; i < static_cast<int>(sizeof(a.u) / 16); ++i) a.u[i] = __ldg(reinterpret_cast<const uint4*>(in + r0) + i);
-  } else {
-#pragma unroll
-    for (int j = 0; j < kIceRows; ++j) a.v[j] = j < cnt ? ld_elem(in + r0 + j) : In{};
-  }
-  uint32_t valid = 0xfu;                                       // r0 is a multiple of 4: the rows share one mask word
-  if (Op::kNullsZero && mask) valid = __ldg(mask + (r0 >> 5)) >> (r0 & 31);
-  RowBuf<Out> b;
-#pragma unroll
-  for (int j = 0; j < kIceRows; ++j) b.v[j] = ((valid >> j) & 1u) ? op(a.v[j]) : Out{};
-  if (vec && cnt == kIceRows) {
-#pragma unroll
-    for (int i = 0; i < static_cast<int>(sizeof(b.u) / 16); ++i) reinterpret_cast<uint4*>(out + r0)[i] = b.u[i];
-  } else {
-#pragma unroll
-    for (int j = 0; j < kIceRows; ++j)
-      if (j < cnt) out[r0 + j] = b.v[j];
-  }
+  map_rows<kIceThreads>(in, mask, out, n, vec, op);
 }
 
 // ---- bytes kernels (STRING / LIST<UINT8>) ------------------------------------------------------------------------------
-// The bytes [0, len) of a row starting at s: word(j) is aligned word j counted from the one holding s[0] (0 when it holds
-// no byte of the row); at(a, b) is the 4 row bytes starting at the first byte of a.
-struct RowWords {
-  const uint32_t* aw;
-  uint32_t sh;        // 8 * (s & 3)
-  int32_t lim;        // (s & 3) + len: word j holds a row byte iff 4j < lim
-  __device__ __forceinline__ RowWords(const uint8_t* s, int32_t len)
-  {
-    aw  = reinterpret_cast<const uint32_t*>(reinterpret_cast<uintptr_t>(s) & ~uintptr_t{3});
-    sh  = 8u * static_cast<uint32_t>(reinterpret_cast<uintptr_t>(s) & 3);
-    lim = static_cast<int32_t>(reinterpret_cast<uintptr_t>(s) & 3) + len;
-  }
-  __device__ __forceinline__ uint32_t word(int32_t j) const { return 4 * j < lim ? __ldg(aw + j) : 0u; }
-  __device__ __forceinline__ uint32_t at(uint32_t a, uint32_t b) const { return __funnelshift_r(a, b, sh); }
-};
-
 // standard murmur3 (seed 0) of len bytes at s; four blocks per step so that their loads are in flight together
 __device__ __forceinline__ uint32_t mm_row(const uint8_t* s, int32_t len)
 {

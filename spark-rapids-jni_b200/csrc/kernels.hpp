@@ -140,6 +140,25 @@ int launch_iceberg_datetime(int32_t transform, const srj_column& in, int32_t* ou
 // stream synchronisation); otherwise *null_count = 0 and out_mask is untouched.
 int launch_decimal128_binary(int32_t op, const srj_column& a, const srj_column& b, int32_t out_scale, bool interim_cast, uint8_t* ovf,
                              void* out, uint32_t* out_mask, int64_t* null_count, cudaStream_t stream);
+// A device counter of the calling host thread on the current device, allocated once; a call that uses it reads it back
+// before it returns.
+int null_counter(unsigned long long** out);
+
+// ---- datetime.cu: DateTimeUtils' rebase and truncation (the caller has checked every argument) ----
+// Truncation formats, in the reference's order of families; TIMESTAMP_DAYS accepts kDtYear .. kDtWeek.
+enum DtFormat : int32_t {
+  kDtYear, kDtQuarter, kDtMonth, kDtWeek, kDtDay, kDtHour, kDtMinute, kDtSecond, kDtMillisecond, kDtMicrosecond, kDtInvalid
+};
+// the format named by len bytes at s (ASCII case-insensitive), kDtInvalid when none
+int32_t datetime_parse_format(const char* s, int32_t len);
+bool datetime_format_fits(int32_t fmt, bool micros);
+// out_mask (NULL: none) gets a copy of the input's mask, all ones when the input has none
+int launch_datetime_rebase(int32_t direction, const srj_column& in, void* out, uint32_t* out_mask, cudaStream_t stream);
+// a format that does not fit the type zeroes out and out_mask (which must then be given); otherwise as the rebase
+int launch_datetime_truncate_scalar(int32_t fmt, const srj_column& in, void* out, uint32_t* out_mask, cudaStream_t stream);
+// fmt.size rows; dt has one row (broadcast) or fmt.size.  Writes out, out_mask and *null_count (one read-back).
+int launch_datetime_truncate_column(const srj_column& dt, const srj_column& fmt, void* out, uint32_t* out_mask, int64_t* null_count,
+                                    cudaStream_t stream);
 
 // ---- kudo.cu: the Kudo shuffle wire format for flat tables (split / assemble) ----
 int64_t kudo_workspace_bytes(int32_t ncols, int32_t P);

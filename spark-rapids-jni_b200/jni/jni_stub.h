@@ -15,7 +15,10 @@ typedef jobject jthrowable;
 typedef jobject jarray;
 typedef jarray jintArray;
 typedef jarray jlongArray;
+typedef jobject jstring;
 struct JNIEnv {
+  const char* GetStringUTFChars(jstring, jboolean*);
+  void ReleaseStringUTFChars(jstring, const char*);
   jclass FindClass(const char*);
   jint ThrowNew(jclass, const char*);
   jboolean ExceptionCheck();

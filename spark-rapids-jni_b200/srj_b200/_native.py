@@ -84,6 +84,9 @@ SYMBOLS = {
     "srj_iceberg_datetime": (C.c_int, [C.c_int32, C.POINTER(SrjColumn), C.c_void_p, C.c_void_p, C.c_void_p]),
     "srj_decimal128_binary": (C.c_int, [C.c_int32, C.POINTER(SrjColumn), C.POINTER(SrjColumn), C.c_int32, C.c_int32, C.c_void_p,
                                         C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
+    "srj_datetime_rebase": (C.c_int, [C.c_int32, C.POINTER(SrjColumn), C.c_void_p, C.c_void_p, C.c_void_p]),
+    "srj_datetime_truncate": (C.c_int, [C.POINTER(SrjColumn), C.POINTER(SrjColumn), C.c_char_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                        C.POINTER(C.c_int64), C.c_void_p]),
     "srj_partition_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int32]),
     "srj_hash_partition": (C.c_int, [C.POINTER(SrjColumn), C.c_int32, C.c_int64, C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
