@@ -413,6 +413,52 @@ SRJ_API int srj_datetime_rebase(int32_t direction, const srj_column* input, void
 SRJ_API int srj_datetime_truncate(const srj_column* datetime, const srj_column* format_col, const char* format, int32_t format_len,
                                   void* out, uint32_t* out_mask, int64_t* null_count, void* stream);
 
+/* ---- JoinPrimitives: hash inner join and the outer / semi / anti gather-map builders --------------------------------
+ * Reference join_primitives.cu:203-227 (hash_inner_join over cudf::hash_join) and 358-576 (the helpers).  Gather maps are
+ * int32 device arrays; INT32_MIN marks the missing side of an outer row.
+ *   srj_hash_join_workspace_bytes : bytes of the join's workspace (build table, per-row counts, tile offsets).
+ *   srj_hash_inner_join_size      : builds a hash table on the right keys, counts every left row's matches and returns the
+ *                                   pair count in *num_pairs (one stream synchronisation).  Keys are equal when every
+ *                                   column is: integers, timestamps, durations and decimals by value, BOOL8 as bool,
+ *                                   FLOAT32 / FLOAT64 with every NaN equal and -0.0 == 0.0, STRING by length and bytes.
+ *                                   With nulls_equal a null equals a null of the same column; without it a row with a null
+ *                                   key matches nothing.  Either side with zero rows: *num_pairs = 0 before any other check.
+ *   srj_hash_inner_join           : (async) with the same arguments and the workspace the size call filled, writes
+ *                                   left_map / right_map (num_pairs each): every pair of rows with equal keys once, the left
+ *                                   map non-decreasing (the order of the right rows of one left row is unspecified).
+ *   SRJ_EINVAL for zero key columns on a side, differing column counts, types or decimal scales, more than INT32_MAX rows,
+ *   columns of one side with differing row counts, a missing or misaligned buffer (data at its element, at most 8 bytes;
+ *   offsets and masks at 4); SRJ_EUNSUPPORTED for LIST / STRUCT (or other non-flat) keys and more than SRJ_MAX_JOIN_KEYS
+ *   key columns.
+ *
+ *   srj_join_mask_workspace_bytes : bytes of one match mask over table_rows rows (a counter, the bitmask, compaction scratch).
+ *   srj_join_mark                 : (async) clears the mask, then sets the bit of every row 0 <= map[i] < table_rows names
+ *                                   and counts the distinct rows set.
+ *   srj_join_matched_counts       : matched[i] = the count of workspaces[i] (one stream synchronisation for all of them).
+ *   srj_join_compact              : (async) out = the ascending rows whose bit is set (matched != 0) or clear (matched == 0).
+ *   srj_join_make_outer           : (async) out_left / out_right = the inner pairs, then every unmatched left row with
+ *                                   INT32_MIN on the right, then (right_ws != NULL: full outer) every unmatched right row with
+ *                                   INT32_MIN on the left.  The workspaces are marked with the maps; left_unmatched /
+ *                                   right_unmatched are the table rows minus their matched counts.
+ *   srj_join_matched_rows         : (async) out[r] (BOOL8, table_rows bytes) = 1 when an in-range map entry names r, else 0.
+ * Maps must be 4-byte aligned; a map may be NULL only when its length is 0.  SRJ_EINVAL for a negative length or table
+ * size, a table size above INT32_MAX, or a missing buffer.  Zero rows touch nothing.
+ */
+#define SRJ_MAX_JOIN_KEYS 32
+SRJ_API int64_t srj_hash_join_workspace_bytes(int64_t left_rows, int64_t right_rows);
+SRJ_API int srj_hash_inner_join_size(const srj_column* left_keys, int32_t num_left_keys, const srj_column* right_keys, int32_t num_right_keys,
+                                     int32_t nulls_equal, int64_t* num_pairs, void* workspace, void* stream);
+SRJ_API int srj_hash_inner_join(const srj_column* left_keys, int32_t num_left_keys, const srj_column* right_keys, int32_t num_right_keys,
+                                int32_t nulls_equal, int32_t* left_map, int32_t* right_map, void* workspace, void* stream);
+SRJ_API int64_t srj_join_mask_workspace_bytes(int64_t table_rows);
+SRJ_API int srj_join_mark(const int32_t* map, int64_t map_len, int64_t table_rows, void* workspace, void* stream);
+SRJ_API int srj_join_matched_counts(const void* const* workspaces, int32_t count, int64_t* matched, void* stream);
+SRJ_API int srj_join_compact(const void* workspace, int64_t table_rows, int32_t matched, int32_t* out, void* stream);
+SRJ_API int srj_join_make_outer(const int32_t* left_map, const int32_t* right_map, int64_t map_len, int64_t left_rows, int64_t right_rows,
+                                const void* left_ws, int64_t left_unmatched, const void* right_ws, int64_t right_unmatched,
+                                int32_t* out_left, int32_t* out_right, void* stream);
+SRJ_API int srj_join_matched_rows(const int32_t* map, int64_t map_len, int64_t table_rows, uint8_t* out, void* stream);
+
 /* ---- multi-GPU configuration (SURVEY 8e: row-range shards + one all-gather of per-column chunks) ---------------- */
 /* ---- Spark HashPartitioning on the device (SURVEY 8f rank 1) ---------------------------------------------------
  * The consumer of Hash.murmurHash32: GpuHashPartitioning computes pmod(murmur3_32(42, keys), P) per row and then

@@ -1205,6 +1205,180 @@ int srj_datetime_truncate(const srj_column* datetime, const srj_column* format_c
 }
 
 // ---------------------------------------------------------------------------------------------------
+// JoinPrimitives: hash inner join and the gather-map helpers (join.cu)
+// ---------------------------------------------------------------------------------------------------
+// join_primitives.cu:212-220 and cudf's validate_hash_join_probe: key counts first, an empty side returns empty, then the
+// schema.  *rows[2] receive the row counts; *empty is set when either is 0 (nothing else was checked then).
+static int join_check(const char* what, const srj_column* l, int32_t nl, const srj_column* r, int32_t nr, int64_t rows[2], bool* empty)
+{
+  if (!l || !r || nl < 0 || nr < 0) { set_error("%s: bad argument", what); return SRJ_EINVAL; }
+  if (nl == 0) { set_error("%s: Left keys table must have at least one column", what); return SRJ_EINVAL; }
+  if (nr == 0) { set_error("%s: Right keys table must have at least one column", what); return SRJ_EINVAL; }
+  for (int side = 0; side < 2; ++side) {
+    const srj_column* t = side ? r : l;
+    const int32_t n     = side ? nr : nl;
+    rows[side]          = t[0].size;
+    for (int32_t c = 0; c < n; ++c)
+      if (t[c].size < 0 || t[c].size != rows[side]) { set_error("%s: the %s key columns have differing or negative row counts", what, side ? "right" : "left"); return SRJ_EINVAL; }
+  }
+  *empty = rows[0] == 0 || rows[1] == 0;
+  if (*empty) return SRJ_OK;
+  for (int side = 0; side < 2; ++side) {
+    const srj_column* t = side ? r : l;
+    for (int32_t c = 0; c < (side ? nr : nl); ++c)
+      if (t[c].type_id != SRJ_STRING && join_key_width(t[c].type_id) == 0) { set_error("%s: key type %d is not supported", what, t[c].type_id); return SRJ_EUNSUPPORTED; }
+  }
+  if (nl != nr) { set_error("%s: Mismatch in number of columns to be joined on", what); return SRJ_EINVAL; }
+  if (nl > SRJ_MAX_JOIN_KEYS) { set_error("%s: more than %d key columns", what, SRJ_MAX_JOIN_KEYS); return SRJ_EUNSUPPORTED; }
+  for (int32_t c = 0; c < nl; ++c)
+    if (l[c].type_id != r[c].type_id || l[c].scale != r[c].scale) { set_error("%s: Mismatch in joining column data types", what); return SRJ_EINVAL; }
+  if (rows[0] > INT32_MAX || rows[1] > INT32_MAX) { set_error("%s: more than INT32_MAX rows", what); return SRJ_EINVAL; }
+  for (int side = 0; side < 2; ++side) {
+    const srj_column* t = side ? r : l;
+    for (int32_t c = 0; c < nl; ++c) {
+      const bool str = t[c].type_id == SRJ_STRING;
+      const int a    = str ? 1 : std::min(join_key_width(t[c].type_id), 8);
+      if ((!t[c].data && !str) || !aligned_to(t[c].data, a) || (str && (!t[c].offsets || !aligned_to(t[c].offsets, 4))) ||
+          !aligned_to(t[c].null_mask, 4)) {
+        set_error("%s: key column %d of the %s table has a missing or misaligned buffer", what, c, side ? "right" : "left");
+        return SRJ_EINVAL;
+      }
+    }
+  }
+  return SRJ_OK;
+}
+
+int64_t srj_hash_join_workspace_bytes(int64_t left_rows, int64_t right_rows)
+{
+  return hash_join_workspace_bytes(std::max<int64_t>(0, left_rows), std::max<int64_t>(0, right_rows));
+}
+
+int srj_hash_inner_join_size(const srj_column* left_keys, int32_t num_left_keys, const srj_column* right_keys, int32_t num_right_keys,
+                             int32_t nulls_equal, int64_t* num_pairs, void* workspace, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "hash_inner_join_size";
+  if (!num_pairs) { set_error("%s: bad argument", what); return SRJ_EINVAL; }
+  int64_t rows[2];
+  bool empty  = false;
+  const int rc = join_check(what, left_keys, num_left_keys, right_keys, num_right_keys, rows, &empty);
+  if (rc != SRJ_OK) return rc;
+  *num_pairs = 0;
+  if (empty) return SRJ_OK;
+  if (!workspace) { set_error("%s: the workspace is needed (srj_hash_join_workspace_bytes)", what); return SRJ_EINVAL; }
+  return launch_hash_join_size(left_keys, right_keys, num_left_keys, rows[0], rows[1], nulls_equal != 0, num_pairs, workspace,
+                               static_cast<cudaStream_t>(stream));
+}
+
+int srj_hash_inner_join(const srj_column* left_keys, int32_t num_left_keys, const srj_column* right_keys, int32_t num_right_keys,
+                        int32_t nulls_equal, int32_t* left_map, int32_t* right_map, void* workspace, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "hash_inner_join";
+  int64_t rows[2];
+  bool empty  = false;
+  const int rc = join_check(what, left_keys, num_left_keys, right_keys, num_right_keys, rows, &empty);
+  if (rc != SRJ_OK || empty) return rc;
+  (void)nulls_equal;   // the size call's counts already hold it
+  if (!workspace || !left_map || !right_map || !aligned_to(left_map, 4) || !aligned_to(right_map, 4)) {
+    set_error("%s: a missing or misaligned map or workspace", what);
+    return SRJ_EINVAL;
+  }
+  return launch_hash_join(left_keys, right_keys, num_left_keys, rows[0], rows[1], left_map, right_map, workspace, static_cast<cudaStream_t>(stream));
+}
+
+// a gather map of map_len entries (4-byte aligned; NULL only when empty) over a table of table_rows rows
+static int join_check_map(const char* what, const int32_t* map, int64_t map_len, int64_t table_rows)
+{
+  if (map_len < 0 || table_rows < 0) { set_error("%s: Table sizes must be non-negative", what); return SRJ_EINVAL; }
+  if (table_rows > INT32_MAX) { set_error("%s: more than INT32_MAX table rows", what); return SRJ_EINVAL; }
+  if ((map_len > 0 && !map) || !aligned_to(map, 4)) { set_error("%s: the gather map is missing or not 4-byte aligned", what); return SRJ_EINVAL; }
+  return SRJ_OK;
+}
+
+int64_t srj_join_mask_workspace_bytes(int64_t table_rows) { return join_mask_workspace_bytes(std::max<int64_t>(0, table_rows)); }
+
+int srj_join_mark(const int32_t* map, int64_t map_len, int64_t table_rows, void* workspace, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "join_mark";
+  const int rc     = join_check_map(what, map, map_len, table_rows);
+  if (rc != SRJ_OK) return rc;
+  if (!workspace || !aligned_to(workspace, 8)) { set_error("%s: the workspace is missing or not 8-byte aligned", what); return SRJ_EINVAL; }
+  return launch_join_mark(map, map_len, table_rows, workspace, static_cast<cudaStream_t>(stream));
+}
+
+int srj_join_matched_counts(const void* const* workspaces, int32_t count, int64_t* matched, void* stream)
+{
+  SRJ_API_RANGE();
+  if (count < 0 || (count > 0 && (!workspaces || !matched))) { set_error("join_matched_counts: bad argument"); return SRJ_EINVAL; }
+  for (int32_t i = 0; i < count; ++i)
+    if (!workspaces[i]) { set_error("join_matched_counts: workspace %d is null", i); return SRJ_EINVAL; }
+  if (count == 0) return SRJ_OK;
+  return read_join_matched(workspaces, count, matched, static_cast<cudaStream_t>(stream));
+}
+
+int srj_join_compact(const void* workspace, int64_t table_rows, int32_t matched, int32_t* out, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "join_compact";
+  const int rc     = join_check_map(what, nullptr, 0, table_rows);
+  if (rc != SRJ_OK) return rc;
+  if (table_rows == 0) return SRJ_OK;
+  if (!workspace || !out || !aligned_to(out, 4)) { set_error("%s: a missing workspace or a missing or misaligned output", what); return SRJ_EINVAL; }
+  return launch_join_compact(workspace, table_rows, matched != 0, out, static_cast<cudaStream_t>(stream));
+}
+
+// join_primitives.cu:358-461
+int srj_join_make_outer(const int32_t* left_map, const int32_t* right_map, int64_t map_len, int64_t left_rows, int64_t right_rows,
+                        const void* left_ws, int64_t left_unmatched, const void* right_ws, int64_t right_unmatched, int32_t* out_left,
+                        int32_t* out_right, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "join_make_outer";
+  int rc           = join_check_map(what, left_map, map_len, left_rows);
+  if (rc != SRJ_OK || (rc = join_check_map(what, right_map, map_len, right_rows)) != SRJ_OK) return rc;
+  const bool full = right_ws != nullptr;
+  if (left_unmatched < 0 || left_unmatched > left_rows || (full && (right_unmatched < 0 || right_unmatched > right_rows))) {
+    set_error("%s: unmatched counts outside the table sizes", what);
+    return SRJ_EINVAL;
+  }
+  const int64_t total = map_len + left_unmatched + (full ? right_unmatched : 0);
+  if (total == 0) return SRJ_OK;
+  if (!left_ws || !out_left || !out_right || !aligned_to(out_left, 4) || !aligned_to(out_right, 4)) {
+    set_error("%s: a missing workspace or a missing or misaligned output", what);
+    return SRJ_EINVAL;
+  }
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (map_len > 0) {
+    SRJ_CUDA_TRY(cudaMemcpyAsync(out_left, left_map, static_cast<size_t>(map_len) * 4, cudaMemcpyDeviceToDevice, s));
+    SRJ_CUDA_TRY(cudaMemcpyAsync(out_right, right_map, static_cast<size_t>(map_len) * 4, cudaMemcpyDeviceToDevice, s));
+  }
+  if (left_unmatched > 0) {
+    if ((rc = launch_join_compact(left_ws, left_rows, false, out_left + map_len, s)) != SRJ_OK) return rc;
+    if ((rc = launch_join_fill(out_right + map_len, left_unmatched, INT32_MIN, s)) != SRJ_OK) return rc;
+  }
+  if (full && right_unmatched > 0) {
+    const int64_t at = map_len + left_unmatched;
+    if ((rc = launch_join_compact(right_ws, right_rows, false, out_right + at, s)) != SRJ_OK) return rc;
+    if ((rc = launch_join_fill(out_left + at, right_unmatched, INT32_MIN, s)) != SRJ_OK) return rc;
+  }
+  return SRJ_OK;
+}
+
+// join_primitives.cu:549-576
+int srj_join_matched_rows(const int32_t* map, int64_t map_len, int64_t table_rows, uint8_t* out, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "join_matched_rows";
+  const int rc     = join_check_map(what, map, map_len, table_rows);
+  if (rc != SRJ_OK) return rc;
+  if (table_rows == 0) return SRJ_OK;
+  if (!out) { set_error("%s: the output is null", what); return SRJ_EINVAL; }
+  return launch_join_matched_rows(map, map_len, table_rows, out, static_cast<cudaStream_t>(stream));
+}
+
+// ---------------------------------------------------------------------------------------------------
 // Spark HashPartitioning: pmod(murmur3_32(seed, keys), P) + stable partition (partition.cu)
 // ---------------------------------------------------------------------------------------------------
 int64_t srj_partition_workspace_bytes(int64_t num_rows, int32_t num_partitions)

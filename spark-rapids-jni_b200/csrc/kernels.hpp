@@ -160,7 +160,26 @@ int launch_datetime_truncate_scalar(int32_t fmt, const srj_column& in, void* out
 int launch_datetime_truncate_column(const srj_column& dt, const srj_column& fmt, void* out, uint32_t* out_mask, int64_t* null_count,
                                     cudaStream_t stream);
 
+// ---- join.cu: JoinPrimitives' hash inner join and gather-map helpers (the caller has checked every argument) ----
+constexpr int32_t kMaxJoinKeys = SRJ_MAX_JOIN_KEYS;
+int32_t join_key_width(int32_t type_id);      // bytes of a fixed-width key type, 0 for any other
+int64_t hash_join_workspace_bytes(int64_t left_rows, int64_t right_rows);
+// builds the table on the right keys, counts each left row's matches and reads the pair count back (one synchronisation)
+int launch_hash_join_size(const srj_column* left, const srj_column* right, int32_t ncols, int64_t left_rows, int64_t right_rows, bool nulls_equal,
+                          int64_t* num_pairs, void* workspace, cudaStream_t stream);
+// writes the pairs from the table and counts launch_hash_join_size left in the workspace
+int launch_hash_join(const srj_column* left, const srj_column* right, int32_t ncols, int64_t left_rows, int64_t right_rows, int32_t* left_map,
+                     int32_t* right_map, void* workspace, cudaStream_t stream);
+int64_t join_mask_workspace_bytes(int64_t rows);
+int launch_join_mark(const int32_t* map, int64_t n, int64_t rows, void* workspace, cudaStream_t stream);
+int read_join_matched(const void* const* workspaces, int32_t count, int64_t* matched, cudaStream_t stream);
+int launch_join_compact(const void* workspace, int64_t rows, bool set, int32_t* out, cudaStream_t stream);
+int launch_join_fill(int32_t* out, int64_t n, int32_t value, cudaStream_t stream);
+int launch_join_matched_rows(const int32_t* map, int64_t n, int64_t rows, uint8_t* out, cudaStream_t stream);
+
 // ---- kudo.cu: the Kudo shuffle wire format for flat tables (split / assemble) ----
+// exclusive scan of v[0 .. n] in place by one CTA (n up to a few 10^5); v[n] receives the total
+int launch_i64_scan_small(int64_t* v, int n, cudaStream_t stream);
 int64_t kudo_workspace_bytes(int32_t ncols, int32_t P);
 int launch_kudo_split_sizes(const srj_column* cols, int32_t ncols, int64_t num_rows, const int32_t* d_splits, int32_t P, int64_t* d_part_offsets,
                             int64_t* h_total, void* workspace, cudaStream_t stream);

@@ -146,6 +146,13 @@ __global__ void __launch_bounds__(1024) i64_scan_small_kernel(int64_t* v, int n)
   }
 }
 
+int launch_i64_scan_small(int64_t* v, int n, cudaStream_t stream)
+{
+  i64_scan_small_kernel<<<1, 1024, 0, stream>>>(v, n);
+  SRJ_CUDA_TRY(cudaGetLastError());
+  return SRJ_OK;
+}
+
 __global__ void __launch_bounds__(256) kudo_split_kernel(const KCol* __restrict__ cols, int ncols, const int32_t* __restrict__ splits,
                                                         const int64_t* __restrict__ part_offsets, uint8_t* __restrict__ out)
 {

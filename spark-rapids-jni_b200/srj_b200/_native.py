@@ -87,6 +87,18 @@ SYMBOLS = {
     "srj_datetime_rebase": (C.c_int, [C.c_int32, C.POINTER(SrjColumn), C.c_void_p, C.c_void_p, C.c_void_p]),
     "srj_datetime_truncate": (C.c_int, [C.POINTER(SrjColumn), C.POINTER(SrjColumn), C.c_char_p, C.c_int32, C.c_void_p, C.c_void_p,
                                         C.POINTER(C.c_int64), C.c_void_p]),
+    "srj_hash_join_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int64]),
+    "srj_hash_inner_join_size": (C.c_int, [C.POINTER(SrjColumn), C.c_int32, C.POINTER(SrjColumn), C.c_int32, C.c_int32, C.POINTER(C.c_int64),
+                                           C.c_void_p, C.c_void_p]),
+    "srj_hash_inner_join": (C.c_int, [C.POINTER(SrjColumn), C.c_int32, C.POINTER(SrjColumn), C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.c_void_p]),
+    "srj_join_mask_workspace_bytes": (C.c_int64, [C.c_int64]),
+    "srj_join_mark": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]),
+    "srj_join_matched_counts": (C.c_int, [C.POINTER(C.c_void_p), C.c_int32, C.POINTER(C.c_int64), C.c_void_p]),
+    "srj_join_compact": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p]),
+    "srj_join_make_outer": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
+                                      C.c_void_p, C.c_void_p, C.c_void_p]),
+    "srj_join_matched_rows": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]),
     "srj_partition_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int32]),
     "srj_hash_partition": (C.c_int, [C.POINTER(SrjColumn), C.c_int32, C.c_int64, C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
