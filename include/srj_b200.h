@@ -413,6 +413,53 @@ SRJ_API int srj_datetime_rebase(int32_t direction, const srj_column* input, void
 SRJ_API int srj_datetime_truncate(const srj_column* datetime, const srj_column* format_col, const char* format, int32_t format_len,
                                   void* out, uint32_t* out_mask, int64_t* null_count, void* stream);
 
+/* ---- GpuTimeZoneDB: timestamps to and from a time zone, one zone per row, and ORC's writer -> reader zones -------------
+ * Reference timezones.cu, datetime_utils.cuh:278-588.  A time zone table is the two columns GpuTimeZoneDB.loadData builds,
+ * one row per zone:
+ *   fixed_transitions : LIST<STRUCT<utcInstant INT64, localInstant INT64, offset INT32>> (offsets, children[0] the STRUCT
+ *                       with its three fields as children), seconds: entry 0 is (INT64_MIN, INT64_MIN, the first offset),
+ *                       then one entry per transition, ascending; localInstant is utc + offsetAfter for a gap and utc +
+ *                       offsetBefore for an overlap, offset is offsetAfter.
+ *   dst_rules         : LIST<INT32> (offsets, children[0] the INT32 column) of the same row count: 0 ints, or two rules of
+ *                       (month, dayOfMonthIndicator, dayOfWeek 0 = Monday .. 6 or -1, secondsFromMidnight, offsetBefore,
+ *                       offsetAfter).
+ * A value's seconds s are truncated toward zero.  When the zone has rules and s is above its last instant (localInstant
+ * converting to UTC, utcInstant from UTC), the rules of year(floor(s / 86400)) give the offset; otherwise the last entry
+ * whose instant is <= s.  The result is value -/+ offset in the value's unit, wrapping in int64.
+ *   srj_timezone_convert       : SRJ_TIMEZONE_TO_UTC / FROM_UTC of a TIMESTAMP_SECONDS / MILLISECONDS / MICROSECONDS /
+ *                                NANOSECONDS column in zone tz_index; out has its type and out_mask (ceil(rows / 32) words,
+ *                                may be NULL only when the input has no mask) a copy of its mask (all ones without one).
+ *                                Reads the zone's bounds back (one stream synchronisation), then runs asynchronously.
+ *                                SRJ_EINVAL for a tz_index outside the table, or a zone without entries or with a rule list
+ *                                of other than 0 or 12 ints.
+ *   srj_timezone_convert_multi : one zone per row, for string-to-timestamp casts: seconds (INT64), micros (INT32), invalid
+ *                                (BOOL8 / UINT8), tz_type (UINT8), tz_offset (INT32) and tz_indices (INT32), all of one row
+ *                                count; input masks are not read.  A row is null when invalid; tz_type 1 (a fixed offset)
+ *                                gives seconds - tz_offset, any other the zone tz_indices[row] converted to UTC (null when the
+ *                                index is outside the table or the zone malformed).  Then micros are added with the
+ *                                reference's overflow check; an overflow is null.  out (TIMESTAMP_MICROSECONDS) holds 0 under
+ *                                nulls; out_mask is needed; *null_count is read back (one stream synchronisation).
+ *   srj_orc_convert_timezones  : (async) ORC's SerializationUtils.convertBetweenTimezones of a TIMESTAMP_MICROSECONDS column.
+ *                                Each zone is (transitions INT64 ms, offsets INT32 ms, raw offset ms); NULL transitions and
+ *                                offsets mean a fixed offset.  The offset at a millisecond is an exact match's, else the
+ *                                previous transition's, the raw offset before the first and from the last on.
+ *                                result = us + (w - r') * 1000 with ms = us / 1000 truncated, w the writer's offset at ms, r
+ *                                the reader's, r' the reader's at ms + w - r.  out_mask as srj_timezone_convert.
+ * All: zero rows touch nothing after the host-side checks.  SRJ_EUNSUPPORTED for an input of another type; SRJ_EINVAL for a
+ * table of another layout, mismatched row counts, or a missing or misaligned buffer (data and out at their element,
+ * offsets and masks at 4 bytes).
+ */
+#define SRJ_TIMEZONE_TO_UTC 0
+#define SRJ_TIMEZONE_FROM_UTC 1
+SRJ_API int srj_timezone_convert(int32_t direction, const srj_column* input, const srj_column* fixed_transitions, const srj_column* dst_rules,
+                                 int32_t tz_index, void* out, uint32_t* out_mask, void* stream);
+SRJ_API int srj_timezone_convert_multi(const srj_column* seconds, const srj_column* micros, const srj_column* invalid, const srj_column* tz_type,
+                                       const srj_column* tz_offset, const srj_column* fixed_transitions, const srj_column* dst_rules,
+                                       const srj_column* tz_indices, int64_t* out, uint32_t* out_mask, int64_t* null_count, void* stream);
+SRJ_API int srj_orc_convert_timezones(const srj_column* input, const srj_column* writer_transitions, const srj_column* writer_offsets,
+                                      int32_t writer_raw_offset, const srj_column* reader_transitions, const srj_column* reader_offsets,
+                                      int32_t reader_raw_offset, void* out, uint32_t* out_mask, void* stream);
+
 /* ---- JoinPrimitives: hash inner join and the outer / semi / anti gather-map builders --------------------------------
  * Reference join_primitives.cu:203-227 (hash_inner_join over cudf::hash_join) and 358-576 (the helpers).  Gather maps are
  * int32 device arrays; INT32_MIN marks the missing side of an outer row.

@@ -1205,6 +1205,135 @@ int srj_datetime_truncate(const srj_column* datetime, const srj_column* format_c
 }
 
 // ---------------------------------------------------------------------------------------------------
+// GpuTimeZoneDB: time zone conversions (timezone.cu)
+// ---------------------------------------------------------------------------------------------------
+static bool is_timestamp_64(int32_t t) { return t >= SRJ_TIMESTAMP_SECONDS && t <= SRJ_TIMESTAMP_NANOSECONDS; }
+
+// a flat column of type t (or of either type when t2 >= 0) with rows rows, its data aligned to its element when rows > 0
+static int tz_check_flat(const char* what, const char* name, const srj_column* c, int32_t t, int32_t t2, int64_t rows)
+{
+  if (!c) { set_error("%s: the %s column is null", what, name); return SRJ_EINVAL; }
+  if (c->type_id != t && c->type_id != t2) { set_error("%s: the %s column has type id %d", what, name, c->type_id); return SRJ_EINVAL; }
+  if (c->size != rows) { set_error("%s: the %s column has %lld rows, not %lld", what, name, static_cast<long long>(c->size), static_cast<long long>(rows)); return SRJ_EINVAL; }
+  const int a = size_of_type(c->type_id);
+  if (rows > 0 && (!c->data || !aligned_to(c->data, a))) { set_error("%s: the %s data is missing or not aligned to %d bytes", what, name, a); return SRJ_EINVAL; }
+  return SRJ_OK;
+}
+
+// the two columns of a time zone table (GpuTimeZoneDB.loadData's layout)
+static int tz_check_table(const char* what, const srj_column* fixed, const srj_column* dst)
+{
+  if (!fixed || !dst) { set_error("%s: the time zone table is null", what); return SRJ_EINVAL; }
+  if (fixed->type_id != SRJ_LIST || dst->type_id != SRJ_LIST || fixed->num_children < 1 || !fixed->children || dst->num_children < 1 || !dst->children) {
+    set_error("%s: the time zone table must be LIST<STRUCT<INT64, INT64, INT32>> and LIST<INT32>", what);
+    return SRJ_EINVAL;
+  }
+  if (fixed->size < 0 || fixed->size > INT32_MAX || dst->size != fixed->size) { set_error("%s: the time zone table's columns have mismatched row counts", what); return SRJ_EINVAL; }
+  if (!fixed->offsets || !aligned_to(fixed->offsets, 4) || !dst->offsets || !aligned_to(dst->offsets, 4)) {
+    set_error("%s: the time zone table's list offsets are missing or not 4-byte aligned", what);
+    return SRJ_EINVAL;
+  }
+  const srj_column* s = &fixed->children[0];
+  if (s->type_id != SRJ_STRUCT || s->num_children != 3 || !s->children) { set_error("%s: the transitions must be STRUCT<INT64, INT64, INT32>", what); return SRJ_EINVAL; }
+  static const char* const names[3] = {"utcInstant", "localInstant", "offset"};
+  for (int i = 0; i < 3; ++i) {
+    const int rc = tz_check_flat(what, names[i], &s->children[i], i < 2 ? SRJ_INT64 : SRJ_INT32, -1, s->size);
+    if (rc != SRJ_OK) return rc;
+  }
+  return tz_check_flat(what, "DST rules", &dst->children[0], SRJ_INT32, -1, dst->children[0].size);
+}
+
+// an input of type t with rows > 0 needs its data and out at 8 bytes, and out_mask when it has a mask
+static int tz_check_io(const char* what, const srj_column* in, const void* out, const uint32_t* out_mask)
+{
+  if (in->size < 0) { set_error("%s: bad row count", what); return SRJ_EINVAL; }
+  if (in->size == 0) return SRJ_OK;
+  if (!in->data || !aligned_to(in->data, 8)) { set_error("%s: the input data is missing or not 8-byte aligned", what); return SRJ_EINVAL; }
+  if (!out || !aligned_to(out, 8)) { set_error("%s: the output is missing or not 8-byte aligned", what); return SRJ_EINVAL; }
+  if ((in->null_mask && !out_mask) || (out_mask && !aligned_to(out_mask, 4))) { set_error("%s: the input has a null mask but no 4-byte aligned output mask was given", what); return SRJ_EINVAL; }
+  return SRJ_OK;
+}
+
+// timezones.cu:80-111, 494-539
+int srj_timezone_convert(int32_t direction, const srj_column* input, const srj_column* fixed_transitions, const srj_column* dst_rules,
+                         int32_t tz_index, void* out, uint32_t* out_mask, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "timezone_convert";
+  if (!input) { set_error("%s: bad argument", what); return SRJ_EINVAL; }
+  if (direction != SRJ_TIMEZONE_TO_UTC && direction != SRJ_TIMEZONE_FROM_UTC) { set_error("%s: unknown direction %d", what, direction); return SRJ_EINVAL; }
+  if (!is_timestamp_64(input->type_id)) { set_error("%s: Unsupported timestamp unit for timezone conversion (type id %d)", what, input->type_id); return SRJ_EUNSUPPORTED; }
+  int rc = tz_check_table(what, fixed_transitions, dst_rules);
+  if (rc != SRJ_OK) return rc;
+  if (tz_index < 0 || tz_index >= fixed_transitions->size) {
+    set_error("%s: time zone index %d is outside the table of %lld zones", what, tz_index, static_cast<long long>(fixed_transitions->size));
+    return SRJ_EINVAL;
+  }
+  if ((rc = tz_check_io(what, input, out, out_mask)) != SRJ_OK) return rc;
+  return launch_timezone_convert(direction == SRJ_TIMEZONE_TO_UTC, *input, *fixed_transitions, *dst_rules, tz_index, out, out_mask,
+                                 static_cast<cudaStream_t>(stream));
+}
+
+// timezones.cu:186-240
+int srj_timezone_convert_multi(const srj_column* seconds, const srj_column* micros, const srj_column* invalid, const srj_column* tz_type,
+                               const srj_column* tz_offset, const srj_column* fixed_transitions, const srj_column* dst_rules,
+                               const srj_column* tz_indices, int64_t* out, uint32_t* out_mask, int64_t* null_count, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "timezone_convert_multi";
+  if (!seconds || !null_count) { set_error("%s: bad argument", what); return SRJ_EINVAL; }
+  if (seconds->type_id != SRJ_INT64) { set_error("%s: seconds column must be of type INT64", what); return SRJ_EUNSUPPORTED; }
+  if (micros && micros->type_id != SRJ_INT32) { set_error("%s: microseconds column must be of type INT32", what); return SRJ_EUNSUPPORTED; }
+  const int64_t n = seconds->size;
+  if (n < 0) { set_error("%s: bad row count", what); return SRJ_EINVAL; }
+  int rc = tz_check_table(what, fixed_transitions, dst_rules);
+  if (rc != SRJ_OK) return rc;
+  const srj_column* cols[6] = {seconds, micros, invalid, tz_type, tz_offset, tz_indices};
+  static const char* const names[6] = {"seconds", "microseconds", "invalid", "tz type", "tz offset", "tz indices"};
+  static const int32_t types[6][2] = {{SRJ_INT64, -1}, {SRJ_INT32, -1}, {SRJ_BOOL8, SRJ_UINT8}, {SRJ_UINT8, -1}, {SRJ_INT32, -1}, {SRJ_INT32, -1}};
+  for (int i = 0; i < 6; ++i)
+    if ((rc = tz_check_flat(what, names[i], cols[i], types[i][0], types[i][1], n)) != SRJ_OK) return rc;
+  if (n == 0) {
+    *null_count = 0;
+    return SRJ_OK;
+  }
+  if (!out || !aligned_to(out, 8)) { set_error("%s: the output is missing or not 8-byte aligned", what); return SRJ_EINVAL; }
+  if (!out_mask || !aligned_to(out_mask, 4)) { set_error("%s: the output mask is missing or not 4-byte aligned", what); return SRJ_EINVAL; }
+  const srj_column in[6] = {*seconds, *micros, *invalid, *tz_type, *tz_offset, *tz_indices};
+  return launch_timezone_convert_multi(in, *fixed_transitions, *dst_rules, out, out_mask, null_count, static_cast<cudaStream_t>(stream));
+}
+
+// timezones.cu:380-486; a NULL table is a fixed offset
+int srj_orc_convert_timezones(const srj_column* input, const srj_column* writer_transitions, const srj_column* writer_offsets,
+                              int32_t writer_raw_offset, const srj_column* reader_transitions, const srj_column* reader_offsets,
+                              int32_t reader_raw_offset, void* out, uint32_t* out_mask, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "orc_convert_timezones";
+  if (!input) { set_error("%s: bad argument", what); return SRJ_EINVAL; }
+  if (input->type_id != SRJ_TIMESTAMP_MICROSECONDS) { set_error("%s: Input column must be of type TIMESTAMP_MICROSECONDS", what); return SRJ_EUNSUPPORTED; }
+  const srj_column* tr[2] = {writer_transitions, reader_transitions};
+  const srj_column* of[2] = {writer_offsets, reader_offsets};
+  int32_t rows[2]         = {0, 0};
+  for (int i = 0; i < 2; ++i) {
+    const char* side = i ? "reader" : "writer";
+    if (!tr[i] && !of[i]) continue;
+    if (!tr[i] || !of[i]) { set_error("%s: the %s table needs both its transitions and its offsets", what, side); return SRJ_EINVAL; }
+    if (tr[i]->size < 0 || tr[i]->size > INT32_MAX) { set_error("%s: bad %s table size", what, side); return SRJ_EINVAL; }
+    int rc = tz_check_flat(what, i ? "reader transitions" : "writer transitions", tr[i], SRJ_INT64, -1, tr[i]->size);
+    if (rc == SRJ_OK) rc = tz_check_flat(what, i ? "reader offsets" : "writer offsets", of[i], SRJ_INT32, -1, tr[i]->size);
+    if (rc != SRJ_OK) return rc;
+    rows[i] = static_cast<int32_t>(tr[i]->size);
+  }
+  const int rc = tz_check_io(what, input, out, out_mask);
+  if (rc != SRJ_OK) return rc;
+  auto ptr64 = [&](int i) { return rows[i] ? static_cast<const int64_t*>(tr[i]->data) : nullptr; };
+  auto ptr32 = [&](int i) { return rows[i] ? static_cast<const int32_t*>(of[i]->data) : nullptr; };
+  return launch_orc_convert_timezones(*input, ptr64(0), ptr32(0), rows[0], writer_raw_offset, ptr64(1), ptr32(1), rows[1], reader_raw_offset, out,
+                                      out_mask, static_cast<cudaStream_t>(stream));
+}
+
+// ---------------------------------------------------------------------------------------------------
 // JoinPrimitives: hash inner join and the gather-map helpers (join.cu)
 // ---------------------------------------------------------------------------------------------------
 // join_primitives.cu:212-220 and cudf's validate_hash_join_probe: key counts first, an empty side returns empty, then the

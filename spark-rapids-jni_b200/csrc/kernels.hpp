@@ -160,6 +160,17 @@ int launch_datetime_truncate_scalar(int32_t fmt, const srj_column& in, void* out
 int launch_datetime_truncate_column(const srj_column& dt, const srj_column& fmt, void* out, uint32_t* out_mask, int64_t* null_count,
                                     cudaStream_t stream);
 
+// ---- timezone.cu: GpuTimeZoneDB's conversions (the caller has checked every argument and the table's layout) ----
+// reads the zone's bounds back (one synchronisation), checks it has an entry and 0 or 12 rule integers, then launches
+int launch_timezone_convert(bool to_utc, const srj_column& in, const srj_column& fixed, const srj_column& dst, int32_t tz_index, void* out,
+                            uint32_t* out_mask, cudaStream_t stream);
+// in[0..5]: seconds, micros, invalid, tz type, tz offset, tz indices.  Writes out, out_mask and *null_count (one read-back).
+int launch_timezone_convert_multi(const srj_column* in, const srj_column& fixed, const srj_column& dst, int64_t* out, uint32_t* out_mask,
+                                  int64_t* null_count, cudaStream_t stream);
+// a table of 0 transitions is a fixed offset (its pointers may be NULL)
+int launch_orc_convert_timezones(const srj_column& in, const int64_t* wt, const int32_t* wo, int32_t wn, int32_t wraw, const int64_t* rt,
+                                 const int32_t* ro, int32_t rn, int32_t rraw, void* out, uint32_t* out_mask, cudaStream_t stream);
+
 // ---- join.cu: JoinPrimitives' hash inner join and gather-map helpers (the caller has checked every argument) ----
 constexpr int32_t kMaxJoinKeys = SRJ_MAX_JOIN_KEYS;
 int32_t join_key_width(int32_t type_id);      // bytes of a fixed-width key type, 0 for any other

@@ -1,5 +1,6 @@
 // map_rows.cuh -- the per-thread body of the fixed-width map kernels (iceberg.cu's ice_map_kernel, datetime.cu's
-// dt_map_kernel), and RowWords, the aligned word reader of a STRING row.
+// dt_map_kernel, timezone.cu's grid-stride tz_convert_kernel / orc_tz_kernel), and RowWords, the aligned word reader of a
+// STRING row.
 #pragma once
 
 #include <stdint.h>
@@ -19,16 +20,15 @@ union RowBuf {
   uint4 u[sizeof(T) * kMapRows / 16];
 };
 
-// One thread of a map over n rows: rows [r0, r0 + kMapRows) with r0 = (block * kThreads + thread) * kMapRows, loaded and
-// stored with 16-byte accesses when vec (both buffers 16-byte aligned) and the thread owns a full group.  With
-// Op::kNullsZero a null row gets Out{} instead of op(v).  Op supplies In, Out and a const operator().
-template <int kThreads, class Op>
-__device__ __forceinline__ void map_rows(const typename Op::In* __restrict__ in, const uint32_t* __restrict__ mask,
-                                         typename Op::Out* __restrict__ out, int64_t n, bool vec, const Op& op)
+// One thread's rows [r0, r0 + kMapRows) of a map over n rows (r0 a multiple of kMapRows), loaded and stored with 16-byte
+// accesses when vec (both buffers 16-byte aligned) and the thread owns a full group.  With Op::kNullsZero a null row gets
+// Out{} instead of op(v).  Op supplies In, Out and a const operator().
+template <class Op>
+__device__ __forceinline__ void map_rows_at(int64_t r0, const typename Op::In* __restrict__ in, const uint32_t* __restrict__ mask,
+                                            typename Op::Out* __restrict__ out, int64_t n, bool vec, const Op& op)
 {
   using In         = typename Op::In;
   using Out        = typename Op::Out;
-  const int64_t r0 = (static_cast<int64_t>(blockIdx.x) * kThreads + threadIdx.x) * kMapRows;
   if (r0 >= n) return;
   const int cnt = static_cast<int>(tmin<int64_t>(kMapRows, n - r0));
   RowBuf<In> a;
@@ -52,6 +52,14 @@ __device__ __forceinline__ void map_rows(const typename Op::In* __restrict__ in,
     for (int j = 0; j < kMapRows; ++j)
       if (j < cnt) out[r0 + j] = b.v[j];
   }
+}
+
+// One thread of a map over n rows, one group per thread: r0 = (block * kThreads + thread) * kMapRows.
+template <int kThreads, class Op>
+__device__ __forceinline__ void map_rows(const typename Op::In* __restrict__ in, const uint32_t* __restrict__ mask,
+                                         typename Op::Out* __restrict__ out, int64_t n, bool vec, const Op& op)
+{
+  map_rows_at((static_cast<int64_t>(blockIdx.x) * kThreads + threadIdx.x) * kMapRows, in, mask, out, n, vec, op);
 }
 
 // The bytes [0, len) of a row starting at s: word(j) is aligned word j counted from the one holding s[0] (0 when it holds

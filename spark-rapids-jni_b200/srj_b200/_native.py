@@ -87,6 +87,11 @@ SYMBOLS = {
     "srj_datetime_rebase": (C.c_int, [C.c_int32, C.POINTER(SrjColumn), C.c_void_p, C.c_void_p, C.c_void_p]),
     "srj_datetime_truncate": (C.c_int, [C.POINTER(SrjColumn), C.POINTER(SrjColumn), C.c_char_p, C.c_int32, C.c_void_p, C.c_void_p,
                                         C.POINTER(C.c_int64), C.c_void_p]),
+    "srj_timezone_convert": (C.c_int, [C.c_int32, C.POINTER(SrjColumn), C.POINTER(SrjColumn), C.POINTER(SrjColumn), C.c_int32, C.c_void_p,
+                                       C.c_void_p, C.c_void_p]),
+    "srj_timezone_convert_multi": (C.c_int, [C.POINTER(SrjColumn)] * 8 + [C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
+    "srj_orc_convert_timezones": (C.c_int, [C.POINTER(SrjColumn), C.POINTER(SrjColumn), C.POINTER(SrjColumn), C.c_int32, C.POINTER(SrjColumn),
+                                            C.POINTER(SrjColumn), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "srj_hash_join_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int64]),
     "srj_hash_inner_join_size": (C.c_int, [C.POINTER(SrjColumn), C.c_int32, C.POINTER(SrjColumn), C.c_int32, C.c_int32, C.POINTER(C.c_int64),
                                            C.c_void_p, C.c_void_p]),
