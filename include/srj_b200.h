@@ -460,6 +460,48 @@ SRJ_API int srj_orc_convert_timezones(const srj_column* input, const srj_column*
                                       int32_t writer_raw_offset, const srj_column* reader_transitions, const srj_column* reader_offsets,
                                       int32_t reader_raw_offset, void* out, uint32_t* out_mask, void* stream);
 
+/* ---- CastStrings: string to timestamp (first phase) and string to date -------------------------------------------------
+ * Reference cast_string_to_datetime.cu (Spark 3.5's SparkDateTimeUtils).  Both trim bytes <= 32 and 127 from each end.
+ *   srj_cast_parse_timestamps : (async) parses [+-]yyyy[y][y][-m[m][-d[d][( |T)[h]h:[m]m:[s]s[.fraction][zone]]]], or a
+ *                               time alone ("T..." or "h:m..."), into the six columns of CastStrings'
+ *                               parseTimestampStringsToIntermediate, one row per input row:
+ *                               result UINT8 (0 ok, 1 invalid), seconds INT64 (the local date-time as seconds from the
+ *                               epoch), micros INT32 (the first 6 fraction digits), tz_type UINT8 (0 none, 1 fixed, 2 other,
+ *                               3 invalid), tz_offset INT32 (seconds, fixed zones), tz_index INT32 (-1 when none).
+ *                               Zones: Z; [+-]h[h], [+-]hh[mm[ss]], [+-]h[h]:m[m], [+-]h[h]:mm:ss up to 18:00:00; UT, UTC,
+ *                               GMT, GMT0 and those prefixes followed by an offset; any other name is looked up in
+ *                               tz_name_map, a STRUCT<name STRING, index INT32> sorted by name bytes (further fields are
+ *                               ignored), and a name it lacks makes the row invalid.  A row without a zone takes type 2 and
+ *                               default_tz_index.  A time alone takes its date from default_epoch_day without a zone, from
+ *                               now_seconds + offset with a fixed zone, and from now_seconds converted into a named zone with
+ *                               the time zone table (fixed_transitions / dst_rules, the layout of srj_timezone_convert).
+ *                               The version (spark_platform 0 = vanilla Spark, 1 = Databricks) selects Spark 3.2.0's
+ *                               offsets (a one-digit minute is rejected, "+hh:mm" right after the time is read with a sign
+ *                               of 1 for '+' and 0 for '-') and, from Spark 4.0 / Databricks 14.3, rejects spaces before
+ *                               "Thh:mm:ss".  Years outside [-300000, 300000] and invalid dates or times are invalid.
+ *                               A null row is invalid (0, 0, 0 and -1 elsewhere) whatever bytes its offsets span.
+ *                               Defined where the reference's is not: a default_tz_index outside the table is SRJ_EINVAL;
+ *                               a time alone whose named zone maps outside the table, or to a malformed zone, is invalid;
+ *                               a tenth segment of a Spark 3.2.0 string is dropped.
+ *   srj_cast_parse_dates      : [+-]yyyy[y][y][y][-[m]m[-[d]d[( |T)anything]]] into TIMESTAMP_DAYS.  A row is null when the
+ *                               input row is, when it does not parse, or when its year is outside [-10^7, 10^7] or its day
+ *                               count outside int32.  out holds 0 under nulls; out_mask is needed; *null_count is read back
+ *                               (one stream synchronisation).
+ * Both: zero rows touch nothing after the host-side checks.  A STRING column (the input, the map's names) may have NULL
+ * chars only when its offsets span no byte; such a column with rows is checked by reading its first and last offsets back
+ * (one stream synchronisation, on that path alone).  SRJ_EINVAL for an input that is not STRING, a name map that is
+ * not STRUCT<STRING, INT32>, STRING offsets that span bytes with NULL chars, a time zone table of another layout, or a missing or misaligned buffer (outputs at their
+ * element, masks and offsets at 4 bytes).
+ */
+#define SRJ_SPARK_VANILLA 0
+#define SRJ_SPARK_DATABRICKS 1
+SRJ_API int srj_cast_parse_timestamps(const srj_column* input, const srj_column* tz_name_map, const srj_column* fixed_transitions,
+                                      const srj_column* dst_rules, int32_t default_tz_index, int64_t default_epoch_day, int64_t now_seconds,
+                                      int32_t spark_platform, int32_t spark_major, int32_t spark_minor, int32_t spark_patch,
+                                      uint8_t* out_result, int64_t* out_seconds, int32_t* out_micros, uint8_t* out_tz_type,
+                                      int32_t* out_tz_offset, int32_t* out_tz_index, void* stream);
+SRJ_API int srj_cast_parse_dates(const srj_column* input, int32_t* out, uint32_t* out_mask, int64_t* null_count, void* stream);
+
 /* ---- JoinPrimitives: hash inner join and the outer / semi / anti gather-map builders --------------------------------
  * Reference join_primitives.cu:203-227 (hash_inner_join over cudf::hash_join) and 358-576 (the helpers).  Gather maps are
  * int32 device arrays; INT32_MIN marks the missing side of an outer row.

@@ -67,6 +67,18 @@ __device__ __forceinline__ int32_t days_from_civil(int32_t y, uint32_t m, uint32
   return era * 146097 + static_cast<int32_t>(doe) - 719468;
 }
 
+// days_from_civil with an int64 era term, for every int32 year whose y - 399 does not overflow (the reference's
+// date_time_utils::to_epoch_day): string casts reach years of 6 (timestamps) and 7 (dates) digits
+__device__ __forceinline__ int64_t days_from_civil64(int32_t y, uint32_t m, uint32_t d)
+{
+  y -= m <= 2;
+  const int32_t era  = (y >= 0 ? y : y - 399) / 400;
+  const uint32_t yoe = static_cast<uint32_t>(y - era * 400);                       // [0, 399]
+  const uint32_t doy = (153 * (m > 2 ? m - 3 : m + 9) + 2) / 5 + d - 1;            // [0, 365]
+  const uint32_t doe = yoe * 365 + yoe / 4 - yoe / 100 + doy;                      // [0, 146096]
+  return era * 146097ll + static_cast<int64_t>(doe) - 719468ll;
+}
+
 // Hinnant's days_from_julian: the day count of a date of the Julian calendar
 __device__ __forceinline__ int32_t days_from_julian(int32_t y, uint32_t m, uint32_t d)
 {

@@ -171,6 +171,15 @@ int launch_timezone_convert_multi(const srj_column* in, const srj_column& fixed,
 int launch_orc_convert_timezones(const srj_column& in, const int64_t* wt, const int32_t* wo, int32_t wn, int32_t wraw, const int64_t* rt,
                                  const int32_t* ro, int32_t rn, int32_t rraw, void* out, uint32_t* out_mask, cudaStream_t stream);
 
+// ---- cast_datetime.cu: CastStrings' string-to-timestamp and string-to-date parses (the caller has checked every argument) ----
+// name_map: STRUCT<STRING, INT32>; fixed / dst: the time zone table; default_tz inside the table.  Asynchronous.
+int launch_cast_parse_timestamps(const srj_column& in, const srj_column& name_map, const srj_column& fixed, const srj_column& dst,
+                                 int32_t default_tz, int64_t default_epoch_day, int64_t now, bool is_320, bool is_400, uint8_t* result,
+                                 int64_t* seconds, int32_t* micros, uint8_t* tz_type, int32_t* tz_offset, int32_t* tz_index,
+                                 cudaStream_t stream);
+// writes out, out_mask and *null_count (one read-back)
+int launch_cast_parse_dates(const srj_column& in, int32_t* out, uint32_t* out_mask, int64_t* null_count, cudaStream_t stream);
+
 // ---- join.cu: JoinPrimitives' hash inner join and gather-map helpers (the caller has checked every argument) ----
 constexpr int32_t kMaxJoinKeys = SRJ_MAX_JOIN_KEYS;
 int32_t join_key_width(int32_t type_id);      // bytes of a fixed-width key type, 0 for any other

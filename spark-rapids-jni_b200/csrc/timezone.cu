@@ -18,6 +18,7 @@
 #include "common.cuh"
 #include "kernels.hpp"
 #include "map_rows.cuh"
+#include "tz_eval.cuh"
 
 namespace srj {
 namespace {
@@ -26,79 +27,6 @@ constexpr int kTzThreads     = 256;
 constexpr int32_t kStageMax  = 1024;    // entries of a zone (or of each ORC table) a CTA stages: 12 bytes each
 constexpr int32_t kWinFirst  = 1900;    // the years whose rule thresholds a CTA precomputes: 1900 .. 2200
 constexpr int32_t kWinYears  = 301;
-constexpr int64_t kSecPerDay = 86400;
-
-struct TzRule {
-  int32_t month, dom, dow, time, before, after;
-};
-
-__device__ __forceinline__ TzRule load_rule(const int32_t* p)
-{
-  return TzRule{__ldg(p), __ldg(p + 1), __ldg(p + 2), __ldg(p + 3), __ldg(p + 4), __ldg(p + 5)};
-}
-
-// ---- date_time_utils, step for step: the int32 / uint32 / int64 widths and C's truncating % are the reference's ----------
-__device__ __forceinline__ int64_t tz_epoch_day(int32_t year, int32_t month, int32_t day)
-{
-  const int32_t y    = year - (month <= 2);
-  const int32_t era  = (y >= 0 ? y : y - 399) / 400;
-  const uint32_t yoe = static_cast<uint32_t>(y - era * 400);
-  const uint32_t doy = static_cast<uint32_t>((153 * (month > 2 ? month - 3 : month + 9) + 2) / 5 + day - 1);
-  const uint32_t doe = yoe * 365 + yoe / 4 - yoe / 100 + doy;
-  return era * 146097ll + static_cast<int64_t>(doe) - 719468ll;
-}
-
-__device__ __forceinline__ int32_t tz_days_in_month(int32_t year, int32_t month)
-{
-  if (month == 2) return ((year % 4 == 0 && year % 100 != 0) || year % 400 == 0) ? 29 : 28;
-  return (month == 4 || month == 6 || month == 9 || month == 11) ? 30 : 31;
-}
-
-// 0 = Monday; negative below day INT32_MIN - 8, as the reference's % gives
-__device__ __forceinline__ int64_t tz_weekday(int64_t days) { return (days - (static_cast<int64_t>(INT32_MIN) - 8)) % 7; }
-
-// the year of floor(s / 86400), the day count taken as an int32 as the reference's to_date takes it
-__device__ __forceinline__ int32_t tz_year(int64_t s)
-{
-  int32_t y, m;
-  civil_year_month(static_cast<int32_t>(floor_div_const<kSecPerDay>(s)), &y, &m);
-  return y;
-}
-
-// the UTC second at which rule r takes effect in year
-__device__ __forceinline__ int64_t rule_instant(int32_t year, const TzRule& r)
-{
-  int64_t days;
-  if (r.dom > 0) {
-    days = tz_epoch_day(year, r.month, r.dom);
-    if (r.dow >= 0) days += 6 - (tz_weekday(days) + (6 - r.dow)) % 7;            // next or same weekday
-  } else {
-    days = tz_epoch_day(year, r.month, tz_days_in_month(year, r.month) + 1 + r.dom);
-    if (r.dow >= 0) days -= (tz_weekday(days) + (7 - r.dow)) % 7;                // previous or same weekday
-  }
-  return days * kSecPerDay + r.time - r.before;
-}
-
-// The two thresholds of a year: before t0 the offset is r0.before, from t0 to t1 r0.after, then r1.after.  From UTC they
-// are the rules' instants (get_offset_for_utc_time); to UTC their local times, the gap's later and the overlap's earlier
-// wall clock, chosen by whether rule 0 is a gap (get_offset_for_local_time).
-struct Thresholds {
-  int64_t t0, t1;
-};
-
-template <bool kToUtc>
-__device__ __forceinline__ Thresholds rule_thresholds(int32_t year, const TzRule& r0, const TzRule& r1)
-{
-  const int64_t u0 = rule_instant(year, r0), u1 = rule_instant(year, r1);
-  if (!kToUtc) return Thresholds{u0, u1};
-  const bool gap = r0.after > r0.before;
-  return Thresholds{u0 + (gap ? r0.after : r0.before), u1 + (gap ? r1.before : r1.after)};
-}
-
-__device__ __forceinline__ int32_t rule_offset(int64_t s, const Thresholds& t, const TzRule& r0, const TzRule& r1)
-{
-  return s < t.t0 ? r0.before : s < t.t1 ? r0.after : r1.after;
-}
 
 // the last i in [0, n) with a[i] <= x (0 when none): upper_bound - 1 over an ascending list whose entry 0 is INT64_MIN
 __device__ __forceinline__ int32_t last_le(const int64_t* a, int32_t n, int64_t x)
@@ -187,15 +115,6 @@ __device__ __forceinline__ bool add_micros_overflows(int64_t seconds, int32_t mi
   return false;
 }
 
-struct TzTable {
-  const int32_t* list;     // zones + 1 offsets into the entries
-  const int64_t* local;    // localInstant of every entry
-  const int32_t* off;      // offset of every entry
-  const int32_t* rule_list;
-  const int32_t* rules;
-  int32_t zones;
-};
-
 __global__ void __launch_bounds__(kTzThreads) tz_multi_kernel(const int64_t* __restrict__ sec, const int32_t* __restrict__ us,
                                                               const uint8_t* __restrict__ invalid, const uint8_t* __restrict__ type,
                                                               const int32_t* __restrict__ fixed_off, const int32_t* __restrict__ idx,
@@ -212,33 +131,7 @@ __global__ void __launch_bounds__(kTzThreads) tz_multi_kernel(const int64_t* __r
     if (__ldg(type + r) == 1) {                                   // FIXED_TZ
       conv = static_cast<int64_t>(static_cast<uint64_t>(s) - static_cast<uint64_t>(static_cast<int64_t>(__ldg(fixed_off + r))));
     } else {
-      const int32_t z = __ldg(idx + r);
-      known           = z >= 0 && z < t.zones;
-      int32_t beg = 0, cnt = 0, rb = 0, rc = 0;
-      if (known) {
-        beg = __ldg(t.list + z);
-        cnt = __ldg(t.list + z + 1) - beg;
-        rb  = __ldg(t.rule_list + z);
-        rc  = __ldg(t.rule_list + z + 1) - rb;
-        known = cnt >= 1 && (rc == 0 || rc == 12);
-      }
-      if (known) {
-        const int64_t* inst = t.local + beg;
-        int32_t o;
-        if (rc == 12 && s > __ldg(reinterpret_cast<const long long*>(inst + cnt - 1))) {
-          const TzRule a = load_rule(t.rules + rb), b = load_rule(t.rules + rb + 6);
-          o = rule_offset(s, rule_thresholds<true>(tz_year(s), a, b), a, b);
-        } else {
-          int32_t base = 0, m = cnt;
-          while (m > 1) {
-            const int32_t half = m >> 1;
-            base = __ldg(reinterpret_cast<const long long*>(inst + base + half)) <= s ? base + half : base;
-            m -= half;
-          }
-          o = __ldg(t.off + beg + base);
-        }
-        conv = static_cast<int64_t>(static_cast<uint64_t>(s) - static_cast<uint64_t>(static_cast<int64_t>(o)));
-      }
+      SRJ_ZONE_SHIFT(true, t, __ldg(idx + r), s, known, conv);
     }
     if (known) {
       int64_t v;

@@ -10,35 +10,6 @@ using namespace srjshim;
 
 namespace {
 
-// the two LIST columns of a time zone table as srj_timezone_convert takes them; the descriptors point into the struct itself
-struct TzTable {
-  srj_column fixed{}, dst{}, entries{}, fields[3]{}, rules{};
-};
-
-void to_srj_table(const cudf::table_view& t, TzTable* out)
-{
-  const cudf::column_view trans = t.column(0), dst = t.column(1);
-  out->fixed.type_id = SRJ_LIST;
-  out->fixed.size    = trans.size();
-  const cudf::lists_column_view tl(trans);
-  out->fixed.offsets = const_cast<int32_t*>(tl.offsets().head<int32_t>());
-  const cudf::column_view st = tl.child();
-  out->entries.type_id       = static_cast<int32_t>(st.type().id());
-  out->entries.size          = st.size();
-  for (int i = 0; i < 3 && i < st.num_children(); ++i) out->fields[i] = to_srj(st.child(i));
-  out->entries.children      = out->fields;
-  out->entries.num_children  = st.num_children() < 3 ? st.num_children() : 3;
-  out->fixed.children        = &out->entries;
-  out->fixed.num_children    = 1;
-  out->dst.type_id           = SRJ_LIST;
-  out->dst.size              = dst.size();
-  const cudf::lists_column_view dl(dst);
-  out->dst.offsets      = const_cast<int32_t*>(dl.offsets().head<int32_t>());
-  out->rules            = to_srj(dl.child());
-  out->dst.children     = &out->rules;
-  out->dst.num_children = 1;
-}
-
 jlong convert(JNIEnv* env, int32_t direction, jlong input, jlong tz_info, jint tz_index)
 {
   if (!input || !tz_info) { throw_java(env, "java/lang/NullPointerException", "column is null"); return 0; }   // JNI_NULL_CHECK

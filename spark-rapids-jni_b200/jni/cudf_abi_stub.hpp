@@ -24,7 +24,8 @@ namespace cudf {
 using size_type     = int32_t;
 using bitmask_type  = uint32_t;
 enum class type_id : int32_t { EMPTY = 0, INT8 = 1, UINT8 = 5, INT32 = 3, INT64 = 4, BOOL8 = 11, TIMESTAMP_DAYS = 12, TIMESTAMP_MICROSECONDS = 15,
-                              STRING = 23, LIST = 24, DECIMAL32 = 25, DECIMAL64 = 26, DECIMAL128 = 27 };
+                              STRING = 23, LIST = 24, DECIMAL32 = 25, DECIMAL64 = 26, DECIMAL128 = 27,
+                              STRUCT = 28 };
 struct data_type {
   data_type(type_id id, int32_t scale = 0);
   type_id id() const;
@@ -70,6 +71,8 @@ std::unique_ptr<column> make_lists_column(size_type num_rows, std::unique_ptr<co
                                           size_type null_count, rmm::device_buffer&& null_mask);
 std::unique_ptr<column> make_strings_column(size_type num_rows, std::unique_ptr<column> offsets, rmm::device_buffer&& chars,
                                             size_type null_count, rmm::device_buffer&& null_mask);
+std::unique_ptr<column> make_structs_column(size_type num_rows, std::vector<std::unique_ptr<column>>&& child_columns, size_type null_count,
+                                            rmm::device_buffer&& null_mask, rmm::cuda_stream_view stream);
 rmm::cuda_stream_view get_default_stream();
 namespace jni {
 void auto_set_device(JNIEnv* env);

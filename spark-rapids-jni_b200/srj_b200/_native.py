@@ -92,6 +92,9 @@ SYMBOLS = {
     "srj_timezone_convert_multi": (C.c_int, [C.POINTER(SrjColumn)] * 8 + [C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
     "srj_orc_convert_timezones": (C.c_int, [C.POINTER(SrjColumn), C.POINTER(SrjColumn), C.POINTER(SrjColumn), C.c_int32, C.POINTER(SrjColumn),
                                             C.POINTER(SrjColumn), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "srj_cast_parse_timestamps": (C.c_int, [C.POINTER(SrjColumn)] * 4 + [C.c_int32, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
+                                            C.c_int32] + [C.c_void_p] * 7),
+    "srj_cast_parse_dates": (C.c_int, [C.POINTER(SrjColumn), C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
     "srj_hash_join_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int64]),
     "srj_hash_inner_join_size": (C.c_int, [C.POINTER(SrjColumn), C.c_int32, C.POINTER(SrjColumn), C.c_int32, C.c_int32, C.POINTER(C.c_int64),
                                            C.c_void_p, C.c_void_p]),

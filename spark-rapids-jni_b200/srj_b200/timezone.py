@@ -30,6 +30,14 @@ from . import ColumnVector, ColumnView, DType, Table, _empty, _stream_ptr
 TO_UTC, FROM_UTC = 0, 1       # SRJ_TIMEZONE_*
 FIXED_TZ = 1                  # tz type of a row with a fixed offset (convertTimestampColumnToUTCWithTzCv)
 INT64_MIN = -(2**63)
+# java.time.ZoneId.SHORT_IDS of region zones (EST, HST and MST are fixed offsets a TZif table does not hold)
+SHORT_IDS = {"ACT": "Australia/Darwin", "AET": "Australia/Sydney", "AGT": "America/Argentina/Buenos_Aires", "ART": "Africa/Cairo",
+             "AST": "America/Anchorage", "BET": "America/Sao_Paulo", "BST": "Asia/Dhaka", "CAT": "Africa/Harare", "CNT": "America/St_Johns",
+             "CST": "America/Chicago", "CTT": "Asia/Shanghai", "EAT": "Africa/Addis_Ababa", "ECT": "Europe/Paris",
+             "IET": "America/Indiana/Indianapolis", "IST": "Asia/Kolkata", "JST": "Asia/Tokyo", "MIT": "Pacific/Apia", "NET": "Asia/Yerevan",
+             "NST": "Pacific/Auckland", "PLT": "Asia/Karachi", "PNT": "America/Phoenix", "PRT": "America/Puerto_Rico",
+             "PST": "America/Los_Angeles", "SST": "Pacific/Guadalcanal", "VST": "Asia/Ho_Chi_Minh"}
+UTC_NAMES = ("UTC", "Etc/UTC", "Etc/GMT", "GMT")
 
 
 def _device(*cols):
@@ -237,6 +245,29 @@ class TimeZoneTable:
 
     def index(self, name: str) -> int:
         return self.names.index(name)
+
+    def name_to_index(self) -> dict:
+        """Every name a string may give for a zone of the table -> its index: the zones' own names, the SHORT_IDS whose zone
+        the table holds, and "Z" for the table's UTC zone (GpuTimeZoneDB's zoneIdToTable)."""
+        out = {n: i for i, n in enumerate(self.names)}
+        for short, region in SHORT_IDS.items():
+            if region in out and short not in out:
+                out[short] = out[region]
+        utc = [out[n] for n in UTC_NAMES if n in out]
+        if utc and "Z" not in out:
+            out["Z"] = utc[0]
+        return out
+
+    def name_to_index_map(self, device="cuda") -> ColumnVector:
+        """GpuTimeZoneDB.getTzNameToIndexMap: STRUCT<name STRING, index INT32> sorted by the names' bytes."""
+        items = sorted((n.encode(), i) for n, i in self.name_to_index().items())
+        chars = b"".join(k for k, _ in items)
+        offs = np.concatenate([[0], np.cumsum([len(k) for k, _ in items])]).astype(np.int32)
+        idx = np.array([i for _, i in items], np.int32)
+        names = ColumnVector(DType(DType.STRING), len(items), torch.from_numpy(np.frombuffer(chars, np.uint8).copy()).to(device),
+                             None, torch.from_numpy(offs).to(device), null_count=0)
+        index = ColumnVector(DType(DType.INT32), len(items), torch.from_numpy(idx.view(np.uint8).copy()).to(device), null_count=0)
+        return ColumnVector(DType(DType.STRUCT), len(items), None, None, null_count=0, children=[names, index])
 
     def arrays(self):
         """-> (list offsets, utc, local, offset, rule list offsets, rules) as numpy arrays."""
