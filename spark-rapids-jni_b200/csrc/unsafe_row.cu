@@ -372,6 +372,7 @@ static int ur_upload(const srj_column* cols, int32_t ncols, void* workspace, UrT
 {
   UrCol h[kUrMaxCols];
   int32_t types[kUrMaxCols];
+  if (ncols <= 0 || ncols > kUrMaxCols) return SRJ_EUNSUPPORTED;   // before the type ids are copied into types[]
   for (int c = 0; c < ncols; ++c) types[c] = cols[c].type_id;
   int32_t nstr = 0;
   const int rc = unsafe_row_layout(types, ncols, &t->bitset_bytes, &t->fixed_bytes, &t->ndec, &nstr);
