@@ -14,12 +14,18 @@
 //
 // The modulo by the per-call constant `bits` uses a host-computed reciprocal (reciprocal.cuh: mod_v1 for V1's 31-bit
 // dividends, mod_v2 for V2's 63-bit ones).  No division instruction or subroutine is left in the put / probe loops.
+#include "check.hpp"
 #include "common.cuh"
 #include "hash_device.cuh"
 #include "kernels.hpp"
 #include "reciprocal.cuh"
 
 namespace srj {
+
+struct BloomHeader {
+  int32_t version, num_hashes, seed, num_longs;   // seed is 0 for V1
+};
+
 namespace {
 
 constexpr int kBloomThreads = 256;
@@ -197,12 +203,13 @@ unsigned grid_for(int64_t threads) { return static_cast<unsigned>((threads + kBl
 
 }  // namespace
 
-uint64_t bloom_reciprocal(int32_t version, uint64_t bits)
+// m with x % bits == x - mulhi(x, m) * bits, minus bits once more when that is >= bits (32-bit x for V1, 64-bit for V2)
+static uint64_t bloom_reciprocal(int32_t version, uint64_t bits)
 {
   return version == 1 ? reciprocal_v1(static_cast<uint32_t>(bits)) : reciprocal_v2(bits);
 }
 
-int launch_bloom_init(const BloomHeader& h, uint8_t* buf, cudaStream_t stream)
+static int launch_bloom_init(const BloomHeader& h, uint8_t* buf, cudaStream_t stream)
 {
   const int hdr_words = h.version == 1 ? 3 : 4;
   auto bswap          = [](int32_t v) { return __builtin_bswap32(static_cast<uint32_t>(v)); };
@@ -215,7 +222,7 @@ int launch_bloom_init(const BloomHeader& h, uint8_t* buf, cudaStream_t stream)
   return SRJ_OK;
 }
 
-int launch_bloom_put(const BloomHeader& h, uint8_t* buf, const srj_column& in, cudaStream_t stream)
+static int launch_bloom_put(const BloomHeader& h, uint8_t* buf, const srj_column& in, cudaStream_t stream)
 {
   const int64_t n = in.size;
   if (n == 0) return SRJ_OK;
@@ -234,7 +241,7 @@ int launch_bloom_put(const BloomHeader& h, uint8_t* buf, const srj_column& in, c
   return SRJ_OK;
 }
 
-int launch_bloom_probe(const BloomHeader& h, const uint8_t* buf, const srj_column& in, uint8_t* out, uint32_t* out_mask, cudaStream_t stream)
+static int launch_bloom_probe(const BloomHeader& h, const uint8_t* buf, const srj_column& in, uint8_t* out, uint32_t* out_mask, cudaStream_t stream)
 {
   const int64_t n = in.size;
   if (n == 0) return SRJ_OK;
@@ -258,7 +265,8 @@ int launch_bloom_probe(const BloomHeader& h, const uint8_t* buf, const srj_colum
   return SRJ_OK;
 }
 
-int launch_bloom_merge(const uint8_t* child, int64_t stride, int32_t nfilters, int hdr_bytes, uint8_t* out, int32_t* d_flag, cudaStream_t stream)
+// header copy, header check (*d_flag <- 1 on a mismatch) and the word-wise OR of `nfilters` filters `stride` bytes apart
+static int launch_bloom_merge(const uint8_t* child, int64_t stride, int32_t nfilters, int hdr_bytes, uint8_t* out, int32_t* d_flag, cudaStream_t stream)
 {
   SRJ_CUDA_TRY(cudaMemsetAsync(d_flag, 0, 4, stream));
   if (nfilters > 1) {
@@ -281,3 +289,153 @@ int launch_bloom_merge(const uint8_t* child, int64_t stride, int32_t nfilters, i
 }
 
 }  // namespace srj
+
+// ---- C ABI (include/srj_b200.h) ----
+using namespace srj;
+
+extern "C" {
+
+static int bloom_hdr_bytes(int32_t version) { return version == 2 ? 16 : 12; }   // bloom_filter.hpp:59-63
+
+static int bloom_check_params(const char* what, int32_t version, int32_t num_hashes, int64_t num_longs)
+{
+  if (version != 1 && version != 2) { set_error("%s: Bloom filter version must be 1 or 2 (got %d)", what, version); return SRJ_EINVAL; }
+  if (num_hashes <= 0) { set_error("%s: Bloom filters must have a positive hash count", what); return SRJ_EINVAL; }
+  if (num_longs <= 0) { set_error("%s: Bloom filters must have a positive number of bits", what); return SRJ_EINVAL; }
+  if (bloom_hdr_bytes(version) + 8 * num_longs > INT32_MAX) { set_error("%s: Bloom filter buffer size exceeds int32 range", what); return SRJ_EINVAL; }
+  return SRJ_OK;
+}
+
+// bloom_filter.cu:189-236 + the size checks of put / probe (bloom_filter.cu:340, 459): parse the serialized header of a
+// filter of `bytes` bytes at device address `buf` (one read-back, one stream synchronisation)
+static int bloom_read_header(const char* what, const uint8_t* buf, int64_t bytes, BloomHeader* h, cudaStream_t stream)
+{
+  if (bytes < 12 || !buf) { set_error("%s: Encountered truncated bloom filter", what); return SRJ_EINVAL; }
+  if (reinterpret_cast<uintptr_t>(buf) & 3) { set_error("%s: the filter buffer must be 4-byte aligned", what); return SRJ_EINVAL; }
+  uint32_t raw[4] = {0, 0, 0, 0};
+  SRJ_CUDA_TRY(cudaMemcpyAsync(raw, buf, static_cast<size_t>(std::min<int64_t>(bytes, 16)), cudaMemcpyDeviceToHost, stream));
+  SRJ_CUDA_TRY(cudaStreamSynchronize(stream));
+  const auto be = [](uint32_t v) { return static_cast<int32_t>(__builtin_bswap32(v)); };
+  h->version    = be(raw[0]);
+  if (h->version != 1 && h->version != 2) { set_error("%s: Unexpected bloom filter version %d", what, h->version); return SRJ_EINVAL; }
+  const int hdr = bloom_hdr_bytes(h->version);
+  if (bytes < hdr) { set_error("%s: Encountered truncated bloom filter header", what); return SRJ_EINVAL; }
+  h->num_hashes = be(raw[1]);
+  h->seed       = h->version == 2 ? be(raw[2]) : 0;
+  h->num_longs  = h->version == 2 ? be(raw[3]) : be(raw[2]);
+  if (h->num_longs <= 0) { set_error("%s: Invalid empty bloom filter size", what); return SRJ_EINVAL; }
+  return SRJ_OK;
+}
+
+static int bloom_check_input(const char* what, const srj_column* in)
+{
+  if (!in) { set_error("%s: input is null", what); return SRJ_EINVAL; }
+  if (in->type_id != SRJ_INT64) { set_error("%s: bloom filters take one INT64 column (type id %d)", what, in->type_id); return SRJ_EUNSUPPORTED; }
+  if (in->size < 0 || (in->size > 0 && !in->data)) { set_error("%s: bad input column", what); return SRJ_EINVAL; }
+  return SRJ_OK;
+}
+
+// put / probe: the buffer must be exactly one filter, and V1 indexes with 31-bit positions (bloom_filter.cu:340-359, 459-471)
+static int bloom_check_filter(const char* what, const BloomHeader& h, int64_t bytes)
+{
+  if (bytes != bloom_hdr_bytes(h.version) + 8 * static_cast<int64_t>(h.num_longs)) {
+    set_error("%s: Encountered invalid/mismatched bloom filter buffer data", what);
+    return SRJ_EINVAL;
+  }
+  if (h.version == 1 && 64 * static_cast<int64_t>(h.num_longs) > INT32_MAX) { set_error("%s: V1 bloom filter bit count exceeds int32 range", what); return SRJ_EINVAL; }
+  return SRJ_OK;
+}
+
+int srj_bloom_filter_sizes(int32_t version, int32_t num_hashes, int64_t bits, int32_t* num_longs, int64_t* total_bytes)
+{
+  SRJ_API_RANGE();
+  if (!num_longs || !total_bytes) { set_error("bloom_filter_sizes: bad argument"); return SRJ_EINVAL; }
+  // BloomFilterJni.cpp:40-47: Spark's BitArray holds at most INT32_MAX longs
+  if (bits > static_cast<int64_t>(INT32_MAX) * 64) {
+    set_error("bloom_filter_sizes: bloom filter bit count must be positive and less than or equal to the maximum supported size");
+    return SRJ_EINVAL;
+  }
+  const int64_t longs = bits > 0 ? (bits + 63) / 64 : 0;
+  const int rc        = bloom_check_params("bloom_filter_sizes", version, num_hashes, longs);
+  if (rc != SRJ_OK) return rc;
+  *num_longs   = static_cast<int32_t>(longs);
+  *total_bytes = bloom_hdr_bytes(version) + 8 * longs;
+  return SRJ_OK;
+}
+
+int srj_bloom_filter_init(int32_t version, int32_t num_hashes, int32_t num_longs, int32_t seed, uint8_t* filter, void* stream)
+{
+  SRJ_API_RANGE();
+  const int rc = bloom_check_params("bloom_filter_init", version, num_hashes, num_longs);
+  if (rc != SRJ_OK) return rc;
+  if (check_out("bloom_filter_init", "filter buffer", filter, 4) != SRJ_OK) return SRJ_EINVAL;
+  return launch_bloom_init(BloomHeader{version, num_hashes, version == 2 ? seed : 0, num_longs}, filter, static_cast<cudaStream_t>(stream));
+}
+
+int srj_bloom_filter_put(uint8_t* filter, int64_t filter_bytes, const srj_column* input, void* stream)
+{
+  SRJ_API_RANGE();
+  int rc = bloom_check_input("bloom_filter_put", input);
+  if (rc != SRJ_OK) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  BloomHeader h{};
+  if ((rc = bloom_read_header("bloom_filter_put", filter, filter_bytes, &h, st)) != SRJ_OK) return rc;
+  if ((rc = bloom_check_filter("bloom_filter_put", h, filter_bytes)) != SRJ_OK) return rc;
+  return launch_bloom_put(h, filter, *input, st);
+}
+
+int srj_bloom_filter_probe(const uint8_t* filter, int64_t filter_bytes, const srj_column* input, uint8_t* out, uint32_t* out_mask, void* stream)
+{
+  SRJ_API_RANGE();
+  int rc = bloom_check_input("bloom_filter_probe", input);
+  if (rc != SRJ_OK) return rc;
+  if ((rc = check_out("bloom_filter_probe", "output", out, 1, input->size > 0)) != SRJ_OK) return rc;
+  if ((rc = check_out("bloom_filter_probe", "output mask", out_mask, 1, input->size > 0 && input->null_mask)) != SRJ_OK) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  BloomHeader h{};
+  if ((rc = bloom_read_header("bloom_filter_probe", filter, filter_bytes, &h, st)) != SRJ_OK) return rc;
+  if ((rc = bloom_check_filter("bloom_filter_probe", h, filter_bytes)) != SRJ_OK) return rc;
+  return launch_bloom_probe(h, filter, *input, out, out_mask, st);
+}
+
+int64_t srj_bloom_filter_merge_workspace_bytes(void) { return 16; }
+
+// bloom_filter.cu:374-449.  The stride of the filters is known from the sizes alone (filters_bytes / num_filters), and the
+// header size follows from it (12 + 8 * num_longs is 4 mod 8, 16 + 8 * num_longs is 0 mod 8), so the header check and
+// the OR are enqueued before the first header is read back; header and flag then come back with one synchronisation and
+// the checks run in the reference's order.  On an error `out` holds garbage.
+int srj_bloom_filter_merge(const uint8_t* filters, int64_t filters_bytes, int32_t num_filters, uint8_t* out, void* workspace, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "bloom_filter_merge";
+  if (num_filters <= 0 || filters_bytes < 0 || (filters_bytes > 0 && !filters)) { set_error("%s: bad argument", what); return SRJ_EINVAL; }
+  if (filters_bytes < 12) { set_error("%s: Encountered truncated bloom filter", what); return SRJ_EINVAL; }
+  if (!workspace || !out) { set_error("%s: the output and the workspace are needed", what); return SRJ_EINVAL; }
+  if ((reinterpret_cast<uintptr_t>(filters) | reinterpret_cast<uintptr_t>(out)) & 3) { set_error("%s: the buffers must be 4-byte aligned", what); return SRJ_EINVAL; }
+  cudaStream_t st       = static_cast<cudaStream_t>(stream);
+  const int64_t stride  = filters_bytes / num_filters;
+  const bool launched   = stride * num_filters == filters_bytes && stride >= 16 && stride % 4 == 0 && stride <= INT32_MAX;
+  auto* d_flag          = static_cast<int32_t*>(workspace);
+  if (launched) {
+    const int rc = launch_bloom_merge(filters, stride, num_filters, stride % 8 == 4 ? 12 : 16, out, d_flag, st);
+    if (rc != SRJ_OK) return rc;
+  }
+  int32_t flag    = 0;
+  uint32_t raw[4] = {0, 0, 0, 0};
+  SRJ_CUDA_TRY(cudaMemcpyAsync(raw, filters, static_cast<size_t>(std::min<int64_t>(filters_bytes, 16)), cudaMemcpyDeviceToHost, st));
+  if (launched) SRJ_CUDA_TRY(cudaMemcpyAsync(&flag, d_flag, 4, cudaMemcpyDeviceToHost, st));
+  SRJ_CUDA_TRY(cudaStreamSynchronize(st));
+  const auto be = [](uint32_t v) { return static_cast<int32_t>(__builtin_bswap32(v)); };
+  const int32_t version = be(raw[0]);
+  if (version != 1 && version != 2) { set_error("%s: Unexpected bloom filter version %d", what, version); return SRJ_EINVAL; }
+  const int hdr = bloom_hdr_bytes(version);
+  if (filters_bytes < hdr) { set_error("%s: Encountered truncated bloom filter header", what); return SRJ_EINVAL; }
+  const int64_t num_longs = version == 2 ? be(raw[3]) : be(raw[2]);
+  if (num_longs <= 0) { set_error("%s: Invalid empty bloom filter size", what); return SRJ_EINVAL; }
+  if (filters_bytes != (hdr + 8 * num_longs) * num_filters) { set_error("%s: Encountered invalid/mismatched bloom filter buffer data", what); return SRJ_EINVAL; }
+  if (hdr + 8 * num_longs > INT32_MAX) { set_error("%s: Bloom filter buffer size exceeds int32 range", what); return SRJ_EINVAL; }
+  if (!launched || flag) { set_error("%s: Mismatch of bloom filter parameters", what); return SRJ_EINVAL; }
+  return SRJ_OK;
+}
+
+}  // extern "C"

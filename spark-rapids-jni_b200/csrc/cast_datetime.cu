@@ -14,6 +14,7 @@
 // share a few L1 lines.  The segments live in named registers (a switch on the segment index), never in an array a lane
 // indexes, so nothing spills to local memory.
 #include "civil_date.cuh"
+#include "check.hpp"
 #include "common.cuh"
 #include "kernels.hpp"
 #include "tz_eval.cuh"
@@ -445,7 +446,8 @@ unsigned blocks_for(int64_t n) { return static_cast<unsigned>((n + kCastThreads 
 
 }  // namespace
 
-int launch_cast_parse_timestamps(const srj_column& in, const srj_column& name_map, const srj_column& fixed, const srj_column& dst,
+// name_map: STRUCT<STRING, INT32>; fixed / dst: the time zone table; default_tz inside the table.  Asynchronous.
+static int launch_cast_parse_timestamps(const srj_column& in, const srj_column& name_map, const srj_column& fixed, const srj_column& dst,
                                  int32_t default_tz, int64_t default_epoch_day, int64_t now, bool is_320, bool is_400, uint8_t* result,
                                  int64_t* seconds, int32_t* micros, uint8_t* tz_type, int32_t* tz_offset, int32_t* tz_index,
                                  cudaStream_t stream)
@@ -479,7 +481,8 @@ int launch_cast_parse_timestamps(const srj_column& in, const srj_column& name_ma
   return SRJ_OK;
 }
 
-int launch_cast_parse_dates(const srj_column& in, int32_t* out, uint32_t* out_mask, int64_t* null_count, cudaStream_t stream)
+// writes out, out_mask and *null_count (one read-back)
+static int launch_cast_parse_dates(const srj_column& in, int32_t* out, uint32_t* out_mask, int64_t* null_count, cudaStream_t stream)
 {
   const int64_t n = in.size;
   *null_count     = 0;
@@ -499,3 +502,87 @@ int launch_cast_parse_dates(const srj_column& in, int32_t* out, uint32_t* out_ma
 }
 
 }  // namespace srj
+
+// ---- C ABI (include/srj_b200.h) ----
+using namespace srj;
+
+extern "C" {
+
+// a STRING column: int32 offsets[rows + 1] at 4 bytes.  Its chars may be NULL only when it holds none: a column with rows
+// and NULL chars has its first and last offsets read back (one stream synchronisation, on that path alone) and is
+// SRJ_EINVAL when they span any byte.
+static int cast_check_strings(const char* what, const char* name, const srj_column* c, cudaStream_t stream)
+{
+  if (!c) { set_error("%s: the %s column is null", what, name); return SRJ_EINVAL; }
+  if (c->type_id != SRJ_STRING) { set_error("%s: the %s column must be STRING (type id %d)", what, name, c->type_id); return SRJ_EINVAL; }
+  if (c->size < 0 || c->size > INT32_MAX) { set_error("%s: bad %s row count", what, name); return SRJ_EINVAL; }
+  if (c->size > 0 && check_offsets(what, name, *c) != SRJ_OK) return SRJ_EINVAL;
+  if (c->null_mask && !aligned_to(c->null_mask, 4)) { set_error("%s: the %s null mask is not 4-byte aligned", what, name); return SRJ_EINVAL; }
+  if (c->size > 0 && !c->data) {
+    int32_t ends[2] = {0, 0};
+    SRJ_CUDA_TRY(cudaMemcpyAsync(&ends[0], c->offsets, sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
+    SRJ_CUDA_TRY(cudaMemcpyAsync(&ends[1], c->offsets + c->size, sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
+    SRJ_CUDA_TRY(cudaStreamSynchronize(stream));
+    if (ends[0] != ends[1]) { set_error("%s: the %s column has no chars but its offsets span %d bytes", what, name, ends[1] - ends[0]); return SRJ_EINVAL; }
+  }
+  return SRJ_OK;
+}
+
+// cast_string_to_datetime.cu:870-948, 1110-1133; version.hpp:64-68
+int srj_cast_parse_timestamps(const srj_column* input, const srj_column* tz_name_map, const srj_column* fixed_transitions, const srj_column* dst_rules,
+                              int32_t default_tz_index, int64_t default_epoch_day, int64_t now_seconds, int32_t spark_platform, int32_t spark_major,
+                              int32_t spark_minor, int32_t spark_patch, uint8_t* out_result, int64_t* out_seconds, int32_t* out_micros,
+                              uint8_t* out_tz_type, int32_t* out_tz_offset, int32_t* out_tz_index, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "cast_parse_timestamps";
+  int rc           = cast_check_strings(what, "input", input, static_cast<cudaStream_t>(stream));
+  if (rc != SRJ_OK) return rc;
+  if (!tz_name_map || tz_name_map->type_id != SRJ_STRUCT || tz_name_map->num_children < 2 || !tz_name_map->children || tz_name_map->size < 0) {
+    set_error("%s: the time zone name map must be STRUCT<STRING, INT32>", what);
+    return SRJ_EINVAL;
+  }
+  const srj_column* names = &tz_name_map->children[0];
+  if ((rc = cast_check_strings(what, "time zone name", names, static_cast<cudaStream_t>(stream))) != SRJ_OK) return rc;
+  if (names->size != tz_name_map->size) { set_error("%s: the time zone name map's fields have mismatched row counts", what); return SRJ_EINVAL; }
+  if ((rc = tz_check_flat(what, "time zone index", &tz_name_map->children[1], SRJ_INT32, -1, tz_name_map->size)) != SRJ_OK) return rc;
+  if ((rc = tz_check_table(what, fixed_transitions, dst_rules)) != SRJ_OK) return rc;
+  if (default_tz_index < 0 || default_tz_index >= fixed_transitions->size) {
+    set_error("%s: default time zone index %d is outside the table of %lld zones", what, default_tz_index,
+              static_cast<long long>(fixed_transitions->size));
+    return SRJ_EINVAL;
+  }
+  const int64_t n = input->size;
+  if (n == 0) return SRJ_OK;
+  if ((rc = check_out(what, "result output", out_result, 1)) != SRJ_OK || (rc = check_out(what, "seconds output", out_seconds, 8)) != SRJ_OK ||
+      (rc = check_out(what, "microseconds output", out_micros, 4)) != SRJ_OK || (rc = check_out(what, "tz type output", out_tz_type, 1)) != SRJ_OK ||
+      (rc = check_out(what, "tz offset output", out_tz_offset, 4)) != SRJ_OK || (rc = check_out(what, "tz index output", out_tz_index, 4)) != SRJ_OK)
+    return rc;
+  // is_vanilla_320 and is_vanilla_400_or_later || is_databricks_14_3_or_later
+  const auto ge = [&](int32_t a, int32_t b, int32_t c) {
+    return spark_major > a || (spark_major == a && (spark_minor > b || (spark_minor == b && spark_patch >= c)));
+  };
+  const bool is_320 = spark_platform == SRJ_SPARK_VANILLA && spark_major == 3 && spark_minor == 2 && spark_patch == 0;
+  const bool is_400 = (spark_platform == SRJ_SPARK_VANILLA && ge(4, 0, 0)) || (spark_platform == SRJ_SPARK_DATABRICKS && ge(14, 3, 0));
+  return launch_cast_parse_timestamps(*input, *tz_name_map, *fixed_transitions, *dst_rules, default_tz_index, default_epoch_day, now_seconds, is_320,
+                                      is_400, out_result, out_seconds, out_micros, out_tz_type, out_tz_offset, out_tz_index,
+                                      static_cast<cudaStream_t>(stream));
+}
+
+// cast_string_to_datetime.cu:1034-1106, 1135-1140
+int srj_cast_parse_dates(const srj_column* input, int32_t* out, uint32_t* out_mask, int64_t* null_count, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "cast_parse_dates";
+  if (!null_count) { set_error("%s: bad argument", what); return SRJ_EINVAL; }
+  int rc = cast_check_strings(what, "input", input, static_cast<cudaStream_t>(stream));
+  if (rc != SRJ_OK) return rc;
+  if (input->size == 0) {
+    *null_count = 0;
+    return SRJ_OK;
+  }
+  if ((rc = check_out(what, "output", out, 4)) != SRJ_OK || (rc = check_out_mask(what, true, out_mask)) != SRJ_OK) return rc;
+  return launch_cast_parse_dates(*input, out, out_mask, null_count, static_cast<cudaStream_t>(stream));
+}
+
+}  // extern "C"

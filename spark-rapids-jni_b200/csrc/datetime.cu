@@ -13,11 +13,17 @@
 #include <type_traits>
 
 #include "civil_date.cuh"
+#include "check.hpp"
 #include "common.cuh"
 #include "kernels.hpp"
 #include "map_rows.cuh"
 
 namespace srj {
+
+// Truncation formats, in the reference's order of families; TIMESTAMP_DAYS accepts kDtYear .. kDtWeek.
+enum DtFormat : int32_t {
+  kDtYear, kDtQuarter, kDtMonth, kDtWeek, kDtDay, kDtHour, kDtMinute, kDtSecond, kDtMillisecond, kDtMicrosecond, kDtInvalid
+};
 
 // ---- formats ------------------------------------------------------------------------------------------------------------
 namespace {
@@ -72,7 +78,8 @@ __host__ __device__ __forceinline__ bool format_fits(int32_t fmt, bool micros)
 
 }  // namespace
 
-int32_t datetime_parse_format(const char* s, int32_t len)
+// the format named by len bytes at s (ASCII case-insensitive), kDtInvalid when none
+static int32_t datetime_parse_format(const char* s, int32_t len)
 {
   if (len < 2 || len > 11) return kDtInvalid;
   uint32_t w[3] = {0, 0, 0};
@@ -296,9 +303,8 @@ int launch_trunc_scalar(int32_t fmt, const srj_column& in, void* out, cudaStream
 
 }  // namespace
 
-bool datetime_format_fits(int32_t fmt, bool micros) { return format_fits(fmt, micros); }
-
-int launch_datetime_rebase(int32_t direction, const srj_column& in, void* out, uint32_t* out_mask, cudaStream_t stream)
+// out_mask (NULL: none) gets a copy of the input's mask, all ones when the input has none
+static int launch_datetime_rebase(int32_t direction, const srj_column& in, void* out, uint32_t* out_mask, cudaStream_t stream)
 {
   if (in.size == 0) return SRJ_OK;
   const int rc = copy_mask(in, out_mask, stream);
@@ -311,7 +317,8 @@ int launch_datetime_rebase(int32_t direction, const srj_column& in, void* out, u
                 : launch_map(in, out, RebaseOp<SRJ_DATETIME_JULIAN_TO_GREGORIAN, false>{}, stream);
 }
 
-int launch_datetime_truncate_scalar(int32_t fmt, const srj_column& in, void* out, uint32_t* out_mask, cudaStream_t stream)
+// a format that does not fit the type zeroes out and out_mask (which must then be given); otherwise as the rebase
+static int launch_datetime_truncate_scalar(int32_t fmt, const srj_column& in, void* out, uint32_t* out_mask, cudaStream_t stream)
 {
   const int64_t n = in.size;
   if (n == 0) return SRJ_OK;
@@ -326,7 +333,8 @@ int launch_datetime_truncate_scalar(int32_t fmt, const srj_column& in, void* out
   return micros ? launch_trunc_scalar<true>(fmt, in, out, stream) : launch_trunc_scalar<false>(fmt, in, out, stream);
 }
 
-int launch_datetime_truncate_column(const srj_column& dt, const srj_column& fmt, void* out, uint32_t* out_mask, int64_t* null_count,
+// fmt.size rows; dt has one row (broadcast) or fmt.size.  Writes out, out_mask and *null_count (one read-back).
+static int launch_datetime_truncate_column(const srj_column& dt, const srj_column& fmt, void* out, uint32_t* out_mask, int64_t* null_count,
                                     cudaStream_t stream)
 {
   const int64_t n = fmt.size;
@@ -353,3 +361,69 @@ int launch_datetime_truncate_column(const srj_column& dt, const srj_column& fmt,
 }
 
 }  // namespace srj
+
+// ---- C ABI (include/srj_b200.h) ----
+using namespace srj;
+
+extern "C" {
+
+static bool is_datetime(int32_t t) { return t == SRJ_TIMESTAMP_DAYS || t == SRJ_TIMESTAMP_MICROSECONDS; }
+
+// datetime_rebase.cu:342-372
+int srj_datetime_rebase(int32_t direction, const srj_column* input, void* out, uint32_t* out_mask, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "datetime_rebase";
+  if (!input) { set_error("%s: bad argument", what); return SRJ_EINVAL; }
+  if (direction != SRJ_DATETIME_GREGORIAN_TO_JULIAN && direction != SRJ_DATETIME_JULIAN_TO_GREGORIAN) {
+    set_error("%s: unknown direction %d", what, direction);
+    return SRJ_EINVAL;
+  }
+  if (!is_datetime(input->type_id)) { set_error("%s: The input must be either day or microsecond timestamps to rebase.", what); return SRJ_EUNSUPPORTED; }
+  if (input->size < 0) { set_error("%s: bad row count", what); return SRJ_EINVAL; }
+  if (input->size == 0) return SRJ_OK;
+  int rc = check_data(what, "datetime", *input);
+  if (rc == SRJ_OK) rc = check_out(what, "output", out, type_width(input->type_id));
+  if (rc == SRJ_OK) rc = check_out_mask(what, input->null_mask, out_mask);
+  if (rc != SRJ_OK) return rc;
+  return launch_datetime_rebase(direction, *input, out, out_mask, static_cast<cudaStream_t>(stream));
+}
+
+// datetime_truncate.cu:327-376
+int srj_datetime_truncate(const srj_column* datetime, const srj_column* format_col, const char* format, int32_t format_len, void* out,
+                          uint32_t* out_mask, int64_t* null_count, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "datetime_truncate";
+  if (!datetime || !null_count || (format_col == nullptr) == (format == nullptr) || (format && format_len < 0)) {
+    set_error("%s: bad argument (give exactly one of a format column and a format string, and a null count)", what);
+    return SRJ_EINVAL;
+  }
+  if (!is_datetime(datetime->type_id)) { set_error("%s: The date/time input must be either day or microsecond timestamps.", what); return SRJ_EUNSUPPORTED; }
+  if (format_col && format_col->type_id != SRJ_STRING) { set_error("%s: The format input must be of string type.", what); return SRJ_EUNSUPPORTED; }
+  if (datetime->size < 0 || (format_col && format_col->size < 0)) { set_error("%s: bad row count", what); return SRJ_EINVAL; }
+  if (format_col && datetime->size != 1 && datetime->size != format_col->size) {
+    set_error("%s: The input date/time column must have exactly one row or the same number of rows as the format column.", what);
+    return SRJ_EINVAL;
+  }
+  const int64_t rows = format_col ? format_col->size : datetime->size;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (rows == 0) {
+    *null_count = 0;
+    return SRJ_OK;
+  }
+  int rc = check_data(what, "datetime", *datetime);
+  if (rc == SRJ_OK) rc = check_out(what, "output", out, type_width(datetime->type_id));
+  if (rc != SRJ_OK) return rc;
+  if (format_col) {
+    if ((rc = check_offsets(what, "format", *format_col)) != SRJ_OK || (rc = check_out_mask(what, true, out_mask)) != SRJ_OK) return rc;
+    return launch_datetime_truncate_column(*datetime, *format_col, out, out_mask, null_count, s);
+  }
+  const int32_t fmt = datetime_parse_format(format, format_len);
+  const bool fits   = format_fits(fmt, datetime->type_id == SRJ_TIMESTAMP_MICROSECONDS);
+  if ((rc = check_out_mask(what, !fits || datetime->null_mask, out_mask)) != SRJ_OK) return rc;
+  *null_count = fits ? -1 : rows;
+  return launch_datetime_truncate_scalar(fmt, *datetime, out, out_mask, s);
+}
+
+}  // extern "C"

@@ -15,6 +15,7 @@
 #include <map>
 #include <type_traits>
 
+#include "check.hpp"
 #include "common.cuh"
 #include "decimal_arith.cuh"
 #include "kernels.hpp"
@@ -358,7 +359,7 @@ int null_counter(unsigned long long** out)
   return SRJ_OK;
 }
 
-int launch_decimal128_binary(int32_t op, const srj_column& a, const srj_column& b, int32_t out_scale, bool interim_cast, uint8_t* ovf,
+static int launch_decimal128_binary(int32_t op, const srj_column& a, const srj_column& b, int32_t out_scale, bool interim_cast, uint8_t* ovf,
                              void* out, uint32_t* out_mask, int64_t* null_count, cudaStream_t stream)
 {
   const int64_t n = a.size;
@@ -429,3 +430,63 @@ int launch_decimal128_binary(int32_t op, const srj_column& a, const srj_column& 
 }
 
 }  // namespace srj
+
+// ---- C ABI (include/srj_b200.h) ----
+using namespace srj;
+
+extern "C" {
+
+// The scale combinations whose rows would reach pow_ten's CUDF_UNREACHABLE (k > 76) or divide by a truncated
+// pow_ten(k).as_128_bits() (k > 38) in the reference, path by path; multiply keeps the reference's own
+// check_scale_divisor (decimal_utils.cu:505-510).  Spark's type rules never produce them.
+static const char* decimal_scale_error(int32_t op, int64_t sa, int64_t sb, int64_t so)
+{
+  switch (op) {
+    case SRJ_DECIMAL_MULTIPLY: return so - (sa + sb) > 38 ? "divisor too big" : nullptr;
+    case SRJ_DECIMAL_DIVIDE:
+    case SRJ_DECIMAL_INTEGER_DIVIDE: {
+      const int64_t x = so - (sa - sb);                 // > 0: round by 10^x; < -38: 10^38, then 10^(-x - 38)
+      return x > 38 || x < -38 - 76 ? "the quotient scale needs a power of ten beyond 10^38 (divisor) or 10^76 (multiplier)" : nullptr;
+    }
+    case SRJ_DECIMAL_REMAINDER: {
+      const int64_t ds = so - sb, ns = ds > 0 ? so - sa : sb - sa;
+      return ds > 38 || ds < -76 || ns > 38 || ns < -76 ? "the remainder scale needs a power of ten beyond 10^38 (divisor) or 10^76 (multiplier)"
+                                                        : nullptr;
+    }
+    default: {
+      const int64_t inter = std::min(sa, sb), d = sa - sb;
+      return d > 76 || d < -76 || inter - so > 76 || so - inter > 38 ? "the intermediate scale needs a power of ten beyond 10^38 (divisor) or 10^76 (multiplier)"
+                                                                     : nullptr;
+    }
+  }
+}
+
+// decimal_utils.cu:967-1167 (multiply_decimal128 .. sub_decimal128)
+int srj_decimal128_binary(int32_t op, const srj_column* a, const srj_column* b, int32_t out_scale, int32_t interim_cast, uint8_t* overflow,
+                          void* out, uint32_t* out_mask, int64_t* null_count, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "decimal128_binary";
+  if (!a || !b) { set_error("%s: bad argument", what); return SRJ_EINVAL; }
+  if (op < SRJ_DECIMAL_MULTIPLY || op > SRJ_DECIMAL_SUBTRACT) { set_error("%s: unknown op %d", what, op); return SRJ_EINVAL; }
+  if (a->type_id != SRJ_DECIMAL128 || b->type_id != SRJ_DECIMAL128) { set_error("%s: not a DECIMAL128 column", what); return SRJ_EUNSUPPORTED; }
+  if (a->size < 0 || a->size != b->size) { set_error("%s: inputs have mismatched row counts", what); return SRJ_EINVAL; }
+  if (const char* e = decimal_scale_error(op, a->scale, b->scale, out_scale)) {
+    set_error("%s: scales (%d, %d) -> %d: %s", what, a->scale, b->scale, out_scale, e);
+    return SRJ_EINVAL;
+  }
+  if (a->size == 0) {
+    if (null_count) *null_count = 0;
+    return SRJ_OK;
+  }
+  int rc = check_data(what, "first input", *a);
+  if (rc == SRJ_OK) rc = check_data(what, "second input", *b);
+  if (rc == SRJ_OK) rc = check_out(what, "overflow output", overflow, 1);
+  if (rc == SRJ_OK) rc = check_out(what, "result output", out, 8);
+  if (rc == SRJ_OK) rc = check_out_mask(what, a->null_mask || b->null_mask, out_mask);
+  if (rc != SRJ_OK) return rc;
+  if ((a->null_mask || b->null_mask) && !null_count) { set_error("%s: an input has a null mask but no null count was given", what); return SRJ_EINVAL; }
+  return launch_decimal128_binary(op, *a, *b, out_scale, interim_cast != 0, overflow, out, out_mask, null_count, static_cast<cudaStream_t>(stream));
+}
+
+}  // extern "C"

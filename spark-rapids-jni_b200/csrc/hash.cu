@@ -9,6 +9,7 @@
 #include <algorithm>
 #include <cstdlib>
 #include <type_traits>
+#include "check.hpp"
 #include "common.cuh"
 #include "hash_device.cuh"
 #include "kernels.hpp"
@@ -424,29 +425,13 @@ static int launch_hash_stream(int kind, const HashParams& hp, int64_t num_rows, 
   return SRJ_OK;
 }
 
-static int elem_size(int32_t t)
-{
-  switch (t) {
-    case SRJ_INT8: case SRJ_UINT8: case SRJ_BOOL8: return 1;
-    case SRJ_INT16: case SRJ_UINT16: return 2;
-    case SRJ_INT32: case SRJ_UINT32: case SRJ_FLOAT32: case SRJ_TIMESTAMP_DAYS: case SRJ_DURATION_DAYS:
-    case SRJ_DECIMAL32: return 4;
-    case SRJ_INT64: case SRJ_UINT64: case SRJ_FLOAT64: case SRJ_TIMESTAMP_SECONDS: case SRJ_TIMESTAMP_MILLISECONDS:
-    case SRJ_TIMESTAMP_MICROSECONDS: case SRJ_TIMESTAMP_NANOSECONDS: case SRJ_DURATION_SECONDS:
-    case SRJ_DURATION_MILLISECONDS: case SRJ_DURATION_MICROSECONDS: case SRJ_DURATION_NANOSECONDS:
-    case SRJ_DECIMAL64: return 8;
-    case SRJ_DECIMAL128: return 16;
-    default: return 0;
-  }
-}
-
 int launch_hash(int kind, const srj_column* cols, int32_t num_columns, int64_t num_rows, int64_t seed, void* out,
                 cudaStream_t stream)
 {
   if (num_columns == 0 || num_rows == 0) return SRJ_OK;  // xxhash64.cu:564
   for (int c = 0; c < num_columns; ++c) {
     const int32_t t = cols[c].type_id;
-    const bool ok   = (t == SRJ_STRING) || elem_size(t) > 0;
+    const bool ok   = (t == SRJ_STRING) || type_width(t) > 0;
     if (!ok) { set_error("hash: column %d has unsupported type id %d (nested/dictionary types are not on this path)", c, t); return SRJ_EUNSUPPORTED; }
     if (kind == SRJ_HASH_HIVE && !hash::hive_supported(t)) { set_error("hive_hash: column %d has unsupported type id %d (hive_hash.cu:63-66)", c, t); return SRJ_EUNSUPPORTED; }
     if (cols[c].size != num_rows) { set_error("hash: column %d has %lld rows, expected %lld", c, (long long)cols[c].size, (long long)num_rows); return SRJ_EINVAL; }
@@ -469,10 +454,10 @@ int launch_hash(int kind, const srj_column* cols, int32_t num_columns, int64_t n
         else if (t == SRJ_INT64) kind2 = 2;
       } else {
         if (t == SRJ_INT32 || t == SRJ_UINT32 || t == SRJ_TIMESTAMP_DAYS || t == SRJ_DURATION_DAYS) kind2 = 1;
-        else if (elem_size(t) == 8 && t != SRJ_FLOAT64) kind2 = 2;  // ints, timestamps, durations, DECIMAL64: raw 8 bytes
+        else if (type_width(t) == 8 && t != SRJ_FLOAT64) kind2 = 2;  // ints, timestamps, durations, DECIMAL64: raw 8 bytes
       }
       p.cols[i] = HashCol{static_cast<const uint8_t*>(c.data), c.null_mask, c.offsets, static_cast<int16_t>(t),
-                          static_cast<int16_t>(kind2), elem_size(t)};
+                          static_cast<int16_t>(kind2), type_width(t)};
     }
     // whole chunks of fixed-width keys: the streaming kernel; the kernels below take what is left (tail rows, STRING keys)
     {

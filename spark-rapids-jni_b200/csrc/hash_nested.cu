@@ -16,6 +16,7 @@
 #include <type_traits>
 #include <vector>
 
+#include "check.hpp"
 #include "common.cuh"
 #include "hash_device.cuh"
 #include "kernels.hpp"
@@ -189,14 +190,6 @@ __global__ void __launch_bounds__(256) row_hash_nested_kernel(const HNode* nodes
 }
 
 // ---- host side ---------------------------------------------------------------------------------------------------
-static int elem_size_of(int32_t t)
-{
-  srj_layout l{};
-  int32_t st = 0, sz = 0;
-  if (t == SRJ_STRING || t == SRJ_LIST || t == SRJ_STRUCT) return 0;
-  return srj_compute_layout(&t, 1, &l, &st, &sz) == SRJ_OK ? sz : -1;
-}
-
 // depth rules of the reference: xxhash64.cu:513-543 (a LIST of STRUCT counts one extra level; leaves count 1),
 // hive_hash.cu:441-466 (every LIST / STRUCT level counts 1, leaves 0); murmur has no limit of its own (recursion-free
 // because structs are decomposed up front) -- the xxhash64 rule is applied to it as well.
@@ -244,8 +237,8 @@ static int flatten(int kind, const srj_column& c, bool under_list, std::vector<H
   n.mask    = c.null_mask;
   n.offsets = c.offsets;
   n.type    = c.type_id;
-  n.size    = elem_size_of(c.type_id);
-  if (n.size < 0) { set_error("hash: unsupported type id %d inside a nested column", c.type_id); return SRJ_EUNSUPPORTED; }
+  n.size    = type_width(c.type_id);   // STRING, LIST, STRUCT: 0
+  if (n.size == 0 && c.type_id != SRJ_STRING && c.type_id != SRJ_LIST && c.type_id != SRJ_STRUCT) { set_error("hash: unsupported type id %d inside a nested column", c.type_id); return SRJ_EUNSUPPORTED; }
   if (c.type_id == SRJ_LIST) {
     if (c.num_children != 1 || !c.children || !c.offsets) { set_error("hash: a LIST column needs offsets and one child"); return SRJ_EINVAL; }
     if (kind == SRJ_HASH_MURMUR3_32 && c.children[0].type_id == SRJ_STRUCT) {

@@ -2,12 +2,11 @@
 // srj_convert_to_rows_host): H2D, the device conversion through the same C ABI the device callers use, D2H.
 // Device staging (buffers + streams) comes from a small per-plan pool and is reused: no cudaMalloc / cudaFree /
 // stream creation on the steady-state path.  No kernels here.
-#include <nvtx3/nvToolsExt.h>
-
 #include <algorithm>
 #include <cstring>
 #include <vector>
 
+#include "check.hpp"
 #include "common.cuh"
 #include "kernels.hpp"
 #include "plan.hpp"
@@ -15,11 +14,6 @@
 namespace srj {
 
 namespace {
-
-struct Range {
-  explicit Range(const char* n) { nvtxRangePushA(n); }
-  ~Range() { nvtxRangePop(); }
-};
 
 // RAII lease of one arena of the plan's pool: the first free one, else wait for arena 0.
 struct ArenaLease {
@@ -63,16 +57,6 @@ struct ArenaLease {
 };
 
 size_t align256(size_t v) { return (v + 255) & ~size_t{255}; }
-
-int check_host_cols(const srj_plan* plan, const srj_column* cols, int64_t num_rows, const char* who)
-{
-  if (!plan || (plan->num_columns > 0 && !cols) || num_rows < 0) { set_error("%s: bad argument", who); return SRJ_EINVAL; }
-  for (int c = 0; c < plan->num_columns; ++c) {
-    if (cols[c].type_id != plan->type_ids[c]) { set_error("%s: column %d type %d does not match the plan (%d)", who, c, cols[c].type_id, plan->type_ids[c]); return SRJ_EINVAL; }
-    if (cols[c].size != num_rows) { set_error("%s: column %d has %lld rows, expected %lld", who, c, (long long)cols[c].size, (long long)num_rows); return SRJ_EINVAL; }
-  }
-  return SRJ_OK;
-}
 
 // ---- fixed-width schemas: chunks pipelined over three streams (H2D | kernel | D2H of consecutive chunks overlap) -----
 int from_rows_host_fixed(const srj_plan* plan, ArenaLease& L, const uint8_t* h_rows, int64_t num_rows, srj_column* h_cols,
@@ -243,8 +227,8 @@ int srj_convert_from_rows_host(const srj_plan* plan, const uint8_t* h_rows, cons
                                int64_t num_rows, srj_column* h_cols, int64_t* h_null_counts, int64_t chunk_rows,
                                srj_host_alloc_fn alloc, void* alloc_ctx)
 {
-  Range nv("srj_convert_from_rows_host");
-  int rc = check_host_cols(plan, h_cols, num_rows, "convert_from_rows_host");
+  SRJ_API_RANGE();
+  int rc = check_cols(plan, h_cols, num_rows, "convert_from_rows_host");
   if (rc != SRJ_OK) return rc;
   const int nc = plan->num_columns;
   if (h_null_counts) std::fill(h_null_counts, h_null_counts + nc, 0);
@@ -265,8 +249,8 @@ int srj_convert_to_rows_host(const srj_plan* plan, const srj_column* h_cols, int
                              int32_t max_batches, int32_t* num_batches, int32_t** h_batch_offsets, uint8_t** h_batch_data,
                              srj_host_alloc_fn alloc, void* alloc_ctx)
 {
-  Range nv("srj_convert_to_rows_host");
-  int rc = check_host_cols(plan, h_cols, num_rows, "convert_to_rows_host");
+  SRJ_API_RANGE();
+  int rc = check_cols(plan, h_cols, num_rows, "convert_to_rows_host");
   if (rc != SRJ_OK) return rc;
   if (!batches || !num_batches || max_batches < 1 || !h_batch_offsets || !h_batch_data || !alloc) { set_error("convert_to_rows_host: bad argument"); return SRJ_EINVAL; }
   *num_batches = 0;

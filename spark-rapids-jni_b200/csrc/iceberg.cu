@@ -18,6 +18,7 @@
 #include <type_traits>
 
 #include "civil_date.cuh"
+#include "check.hpp"
 #include "common.cuh"
 #include "hash_device.cuh"
 #include "kernels.hpp"
@@ -344,7 +345,8 @@ const uint8_t* bytes_of(const srj_column& c)
 
 }  // namespace
 
-int launch_iceberg_bucket(const srj_column& in, int32_t num_buckets, int32_t* out, uint32_t* out_mask, cudaStream_t stream)
+// out_mask (NULL: none) gets a copy of the input's mask, all ones when the input has none.
+static int launch_iceberg_bucket(const srj_column& in, int32_t num_buckets, int32_t* out, uint32_t* out_mask, cudaStream_t stream)
 {
   const int64_t n = in.size;
   if (n == 0) return SRJ_OK;
@@ -366,7 +368,7 @@ int launch_iceberg_bucket(const srj_column& in, int32_t num_buckets, int32_t* ou
   }
 }
 
-int launch_iceberg_truncate_fixed(const srj_column& in, int32_t width, void* out, uint32_t* out_mask, cudaStream_t stream)
+static int launch_iceberg_truncate_fixed(const srj_column& in, int32_t width, void* out, uint32_t* out_mask, cudaStream_t stream)
 {
   if (in.size == 0) return SRJ_OK;
   int rc = copy_mask(in, out_mask, stream);
@@ -382,9 +384,10 @@ int launch_iceberg_truncate_fixed(const srj_column& in, int32_t width, void* out
   }
 }
 
-int64_t iceberg_truncate_workspace_bytes(int64_t n) { return 4 * tmax<int64_t>(1, i32_scan_nchunks(n)); }
+static int64_t iceberg_truncate_workspace_bytes(int64_t n) { return 4 * tmax<int64_t>(1, i32_scan_nchunks(n)); }
 
-int launch_iceberg_truncate_sizes(const srj_column& in, int32_t width, int32_t* d_offsets, int64_t* h_total, void* workspace,
+// STRING / LIST<UINT8>: d_offsets[0 .. n] and *h_total (reads the total back: one stream synchronisation)
+static int launch_iceberg_truncate_sizes(const srj_column& in, int32_t width, int32_t* d_offsets, int64_t* h_total, void* workspace,
                                   cudaStream_t stream)
 {
   const int64_t n = in.size;
@@ -405,7 +408,7 @@ int launch_iceberg_truncate_sizes(const srj_column& in, int32_t width, int32_t* 
   return SRJ_OK;
 }
 
-int launch_iceberg_truncate_bytes(const srj_column& in, const int32_t* out_offsets, uint8_t* out_bytes, uint32_t* out_mask, cudaStream_t stream)
+static int launch_iceberg_truncate_bytes(const srj_column& in, const int32_t* out_offsets, uint8_t* out_bytes, uint32_t* out_mask, cudaStream_t stream)
 {
   const int64_t n = in.size;
   if (n == 0) return SRJ_OK;
@@ -416,7 +419,7 @@ int launch_iceberg_truncate_bytes(const srj_column& in, const int32_t* out_offse
   return SRJ_OK;
 }
 
-int launch_iceberg_datetime(int32_t transform, const srj_column& in, int32_t* out, uint32_t* out_mask, cudaStream_t stream)
+static int launch_iceberg_datetime(int32_t transform, const srj_column& in, int32_t* out, uint32_t* out_mask, cudaStream_t stream)
 {
   if (in.size == 0) return SRJ_OK;
   int rc = copy_mask(in, out_mask, stream);
@@ -436,3 +439,124 @@ int launch_iceberg_datetime(int32_t transform, const srj_column& in, int32_t* ou
 }
 
 }  // namespace srj
+
+// ---- C ABI (include/srj_b200.h) ----
+using namespace srj;
+
+extern "C" {
+
+static bool is_binary(const srj_column* c)
+{
+  return c->type_id == SRJ_LIST && c->num_children >= 1 && c->children && c->children[0].type_id == SRJ_UINT8;
+}
+
+// the input's buffers for rows > 0: STRING / LIST offsets, else the data; with check_mask, an input with a mask needs an
+// output mask
+static int ice_check_buffers(const char* what, const srj_column* in, const uint32_t* out_mask, bool check_mask = true)
+{
+  if (in->size < 0) { set_error("%s: bad row count", what); return SRJ_EINVAL; }
+  if (in->size == 0) return SRJ_OK;
+  const int rc = in->type_id == SRJ_STRING || in->type_id == SRJ_LIST ? check_offsets(what, "input", *in) : check_data(what, "input", *in);
+  if (rc != SRJ_OK || !check_mask) return rc;
+  return check_out(what, "output mask", out_mask, 1, in->null_mask != nullptr);
+}
+
+// iceberg_bucket.cu:393, 411-454
+int srj_iceberg_bucket(const srj_column* input, int32_t num_buckets, int32_t* out, uint32_t* out_mask, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "iceberg_bucket";
+  if (!input) { set_error("%s: bad argument", what); return SRJ_EINVAL; }
+  if (num_buckets <= 0) { set_error("%s: num_buckets must be positive", what); return SRJ_EINVAL; }
+  switch (input->type_id) {
+    case SRJ_INT32: case SRJ_INT64: case SRJ_DECIMAL32: case SRJ_DECIMAL64: case SRJ_DECIMAL128:
+    case SRJ_TIMESTAMP_DAYS: case SRJ_TIMESTAMP_MICROSECONDS: case SRJ_STRING: break;
+    case SRJ_LIST:
+      if (is_binary(input)) break;
+      set_error("%s: Binary type must be LIST of UINT8", what);
+      return SRJ_EUNSUPPORTED;
+    default: set_error("%s: Unsupported type for bucket transform: %d", what, input->type_id); return SRJ_EUNSUPPORTED;
+  }
+  int rc = ice_check_buffers(what, input, out_mask);
+  if (rc != SRJ_OK) return rc;
+  if (input->size > 0 && (rc = check_out(what, "output", out, 4)) != SRJ_OK) return rc;
+  return launch_iceberg_bucket(*input, num_buckets, out, out_mask, static_cast<cudaStream_t>(stream));
+}
+
+static bool truncate_integral(int32_t t)
+{
+  return t == SRJ_INT32 || t == SRJ_INT64 || t == SRJ_DECIMAL32 || t == SRJ_DECIMAL64 || t == SRJ_DECIMAL128;
+}
+
+// iceberg_truncate.cu:174-175, 202-213: STRING or LIST<UINT8> with a non-nullable child, width > 0
+static int truncate_bytes_check(const char* what, const srj_column* in, int32_t width)
+{
+  if (in->type_id != SRJ_STRING && in->type_id != SRJ_LIST) { set_error("%s: Unsupported type for truncation", what); return SRJ_EUNSUPPORTED; }
+  if (width <= 0) { set_error("%s: Length must be positive", what); return SRJ_EINVAL; }
+  if (in->type_id == SRJ_LIST) {
+    if (!is_binary(in)) { set_error("%s: Input must be LIST(UINT8)", what); return SRJ_EUNSUPPORTED; }
+    if (in->children[0].null_mask) { set_error("%s: Child column of binary column must be non-nullable", what); return SRJ_EINVAL; }
+  }
+  return SRJ_OK;
+}
+
+int64_t srj_iceberg_truncate_workspace_bytes(int64_t num_rows) { return iceberg_truncate_workspace_bytes(std::max<int64_t>(0, num_rows)); }
+
+int srj_iceberg_truncate_sizes(const srj_column* input, int32_t width, int32_t* d_out_offsets, int64_t* total_bytes, void* workspace,
+                               void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "iceberg_truncate_sizes";
+  if (!input || !d_out_offsets || !total_bytes) { set_error("%s: bad argument", what); return SRJ_EINVAL; }
+  int rc = truncate_bytes_check(what, input, width);
+  if (rc != SRJ_OK) return rc;
+  if ((rc = ice_check_buffers(what, input, nullptr, false)) != SRJ_OK) return rc;
+  if ((rc = check_out(what, "output offsets", d_out_offsets, 4)) != SRJ_OK) return rc;
+  if (input->size > 0 && !workspace) { set_error("%s: the workspace is needed (srj_iceberg_truncate_workspace_bytes)", what); return SRJ_EINVAL; }
+  return launch_iceberg_truncate_sizes(*input, width, d_out_offsets, total_bytes, workspace, static_cast<cudaStream_t>(stream));
+}
+
+// iceberg_truncate.cu:146-166 (integral), IcebergTruncateJni.cpp (the type switch)
+int srj_iceberg_truncate(const srj_column* input, int32_t width, const srj_column* out, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "iceberg_truncate";
+  if (!input || !out) { set_error("%s: bad argument", what); return SRJ_EINVAL; }
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (truncate_integral(input->type_id)) {
+    if (width == 0) { set_error("%s: Width must not be zero", what); return SRJ_EINVAL; }
+    int rc = ice_check_buffers(what, input, out->null_mask);
+    if (rc != SRJ_OK) return rc;
+    if (input->size > 0 && (rc = check_out(what, "output data", out->data, std::min(type_width(input->type_id), 8))) != SRJ_OK) return rc;
+    return launch_iceberg_truncate_fixed(*input, width, out->data, out->null_mask, s);
+  }
+  int rc = truncate_bytes_check(what, input, width);
+  if (rc != SRJ_OK) return rc;
+  if ((rc = ice_check_buffers(what, input, out->null_mask)) != SRJ_OK) return rc;
+  if (input->size == 0) return SRJ_OK;
+  if (!out->offsets) { set_error("%s: the output needs the offsets of srj_iceberg_truncate_sizes", what); return SRJ_EINVAL; }
+  if (input->type_id == SRJ_LIST && (out->num_children < 1 || !out->children)) { set_error("%s: the LIST output needs its UINT8 child", what); return SRJ_EINVAL; }
+  uint8_t* bytes = static_cast<uint8_t*>(input->type_id == SRJ_LIST ? out->children[0].data : out->data);
+  return launch_iceberg_truncate_bytes(*input, out->offsets, bytes, out->null_mask, s);
+}
+
+// iceberg_datetime_util.cu:137-248 and IcebergDateTimeUtil.java's type checks
+int srj_iceberg_datetime(int32_t transform, const srj_column* input, int32_t* out, uint32_t* out_mask, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "iceberg_datetime";
+  if (!input) { set_error("%s: bad argument", what); return SRJ_EINVAL; }
+  if (transform < SRJ_ICEBERG_YEARS || transform > SRJ_ICEBERG_HOURS) { set_error("%s: unknown transform %d", what, transform); return SRJ_EINVAL; }
+  const bool days = input->type_id == SRJ_TIMESTAMP_DAYS, micros = input->type_id == SRJ_TIMESTAMP_MICROSECONDS;
+  if (!micros && !(days && transform != SRJ_ICEBERG_HOURS)) {
+    set_error("%s: Input column must be of type TIMESTAMP_MICROSECONDS%s (type id %d)", what, transform == SRJ_ICEBERG_HOURS ? "" : " or TIMESTAMP_DAYS",
+              input->type_id);
+    return SRJ_EUNSUPPORTED;
+  }
+  int rc = ice_check_buffers(what, input, out_mask);
+  if (rc != SRJ_OK) return rc;
+  if (input->size > 0 && (rc = check_out(what, "output", out, 4)) != SRJ_OK) return rc;
+  return launch_iceberg_datetime(transform, *input, out, out_mask, static_cast<cudaStream_t>(stream));
+}
+
+}  // extern "C"

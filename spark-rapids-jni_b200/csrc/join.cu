@@ -21,6 +21,7 @@
 // join_fill_kernel writes INT32_MIN sentinels; join_matched_rows_kernel writes BOOL8 flags.
 #include <algorithm>
 
+#include "check.hpp"
 #include "common.cuh"
 #include "hash_device.cuh"
 #include "kernels.hpp"
@@ -50,7 +51,7 @@ struct JCol {
   const int32_t* offsets;
 };
 struct JKeys {
-  JCol l[kMaxJoinKeys], r[kMaxJoinKeys];
+  JCol l[SRJ_MAX_JOIN_KEYS], r[SRJ_MAX_JOIN_KEYS];
   int32_t n;
 };
 
@@ -370,7 +371,7 @@ JKeys join_keys(const srj_column* left, const srj_column* right, int32_t n)
       const srj_column& s = side ? right[c] : left[c];
       JCol& d             = side ? k.r[c] : k.l[c];
       d.type              = s.type_id;
-      d.width             = s.type_id == SRJ_STRING ? 0 : join_key_width(s.type_id);
+      d.width             = s.type_id == SRJ_STRING ? 0 : type_width(s.type_id);
       d.data              = static_cast<const uint8_t*>(s.data);
       d.mask              = s.null_mask;
       d.offsets           = s.offsets;
@@ -404,27 +405,14 @@ MaskWs mask_ws(const void* ws, int64_t rows)
 
 }  // namespace
 
-int32_t join_key_width(int32_t type_id)
-{
-  switch (type_id) {
-    case SRJ_INT8: case SRJ_UINT8: case SRJ_BOOL8: return 1;
-    case SRJ_INT16: case SRJ_UINT16: return 2;
-    case SRJ_INT32: case SRJ_UINT32: case SRJ_FLOAT32: case SRJ_TIMESTAMP_DAYS: case SRJ_DURATION_DAYS: case SRJ_DECIMAL32: return 4;
-    case SRJ_INT64: case SRJ_UINT64: case SRJ_FLOAT64: case SRJ_DECIMAL64:
-    case SRJ_TIMESTAMP_SECONDS: case SRJ_TIMESTAMP_MILLISECONDS: case SRJ_TIMESTAMP_MICROSECONDS: case SRJ_TIMESTAMP_NANOSECONDS:
-    case SRJ_DURATION_SECONDS: case SRJ_DURATION_MILLISECONDS: case SRJ_DURATION_MICROSECONDS: case SRJ_DURATION_NANOSECONDS: return 8;
-    case SRJ_DECIMAL128: return 16;
-    default: return 0;
-  }
-}
-
-int64_t hash_join_workspace_bytes(int64_t left_rows, int64_t right_rows)
+static int64_t hash_join_workspace_bytes(int64_t left_rows, int64_t right_rows)
 {
   return round_up64(static_cast<int64_t>(join_buckets(right_rows)) * 32, 256) + round_up64((join_tiles(left_rows) + 1) * 8, 256) +
          round_up64(left_rows * 4, 256);
 }
 
-int launch_hash_join_size(const srj_column* left, const srj_column* right, int32_t ncols, int64_t left_rows, int64_t right_rows, bool nulls_equal,
+// builds the table on the right keys, counts each left row's matches and reads the pair count back (one synchronisation)
+static int launch_hash_join_size(const srj_column* left, const srj_column* right, int32_t ncols, int64_t left_rows, int64_t right_rows, bool nulls_equal,
                           int64_t* num_pairs, void* workspace, cudaStream_t stream)
 {
   const JKeys k         = join_keys(left, right, ncols);
@@ -445,7 +433,8 @@ int launch_hash_join_size(const srj_column* left, const srj_column* right, int32
   return SRJ_OK;
 }
 
-int launch_hash_join(const srj_column* left, const srj_column* right, int32_t ncols, int64_t left_rows, int64_t right_rows, int32_t* left_map,
+// writes the pairs from the table and counts launch_hash_join_size left in the workspace
+static int launch_hash_join(const srj_column* left, const srj_column* right, int32_t ncols, int64_t left_rows, int64_t right_rows, int32_t* left_map,
                      int32_t* right_map, void* workspace, cudaStream_t stream)
 {
   const JKeys k     = join_keys(left, right, ncols);
@@ -457,13 +446,13 @@ int launch_hash_join(const srj_column* left, const srj_column* right, int32_t nc
   return SRJ_OK;
 }
 
-int64_t join_mask_workspace_bytes(int64_t rows)
+static int64_t join_mask_workspace_bytes(int64_t rows)
 {
   const int64_t tiles = mask_tiles(rows);
   return 256 + round_up64((rows + 31) / 32 * 4, 256) + round_up64(tiles * 4, 256) + round_up64(i32_scan_nchunks(tiles) * 4, 256);
 }
 
-int launch_join_mark(const int32_t* map, int64_t n, int64_t rows, void* workspace, cudaStream_t stream)
+static int launch_join_mark(const int32_t* map, int64_t n, int64_t rows, void* workspace, cudaStream_t stream)
 {
   const MaskWs m = mask_ws(workspace, rows);
   SRJ_CUDA_TRY(cudaMemsetAsync(m.matched, 0, 256 + (rows + 31) / 32 * 4, stream));   // the counter, its padding and the mask
@@ -473,7 +462,7 @@ int launch_join_mark(const int32_t* map, int64_t n, int64_t rows, void* workspac
   return SRJ_OK;
 }
 
-int read_join_matched(const void* const* workspaces, int32_t count, int64_t* matched, cudaStream_t stream)
+static int read_join_matched(const void* const* workspaces, int32_t count, int64_t* matched, cudaStream_t stream)
 {
   for (int32_t i = 0; i < count; ++i)
     SRJ_CUDA_TRY(cudaMemcpyAsync(matched + i, workspaces[i], sizeof(int64_t), cudaMemcpyDeviceToHost, stream));
@@ -481,7 +470,7 @@ int read_join_matched(const void* const* workspaces, int32_t count, int64_t* mat
   return SRJ_OK;
 }
 
-int launch_join_compact(const void* workspace, int64_t rows, bool set, int32_t* out, cudaStream_t stream)
+static int launch_join_compact(const void* workspace, int64_t rows, bool set, int32_t* out, cudaStream_t stream)
 {
   if (rows == 0) return SRJ_OK;
   const MaskWs m      = mask_ws(workspace, rows);
@@ -495,7 +484,7 @@ int launch_join_compact(const void* workspace, int64_t rows, bool set, int32_t* 
   return SRJ_OK;
 }
 
-int launch_join_fill(int32_t* out, int64_t n, int32_t value, cudaStream_t stream)
+static int launch_join_fill(int32_t* out, int64_t n, int32_t value, cudaStream_t stream)
 {
   if (n == 0) return SRJ_OK;
   join_fill_kernel<<<blocks_for(n, kJoinThreads), kJoinThreads, 0, stream>>>(out, n, value);
@@ -503,7 +492,7 @@ int launch_join_fill(int32_t* out, int64_t n, int32_t value, cudaStream_t stream
   return SRJ_OK;
 }
 
-int launch_join_matched_rows(const int32_t* map, int64_t n, int64_t rows, uint8_t* out, cudaStream_t stream)
+static int launch_join_matched_rows(const int32_t* map, int64_t n, int64_t rows, uint8_t* out, cudaStream_t stream)
 {
   if (rows == 0) return SRJ_OK;
   SRJ_CUDA_TRY(cudaMemsetAsync(out, 0, static_cast<size_t>(rows), stream));
@@ -514,3 +503,172 @@ int launch_join_matched_rows(const int32_t* map, int64_t n, int64_t rows, uint8_
 }
 
 }  // namespace srj
+
+// ---- C ABI (include/srj_b200.h) ----
+using namespace srj;
+
+extern "C" {
+
+// join_primitives.cu:212-220 and cudf's validate_hash_join_probe: key counts first, an empty side returns empty, then the
+// schema.  *rows[2] receive the row counts; *empty is set when either is 0 (nothing else was checked then).
+static int join_check(const char* what, const srj_column* l, int32_t nl, const srj_column* r, int32_t nr, int64_t rows[2], bool* empty)
+{
+  if (!l || !r || nl < 0 || nr < 0) { set_error("%s: bad argument", what); return SRJ_EINVAL; }
+  if (nl == 0) { set_error("%s: Left keys table must have at least one column", what); return SRJ_EINVAL; }
+  if (nr == 0) { set_error("%s: Right keys table must have at least one column", what); return SRJ_EINVAL; }
+  for (int side = 0; side < 2; ++side) {
+    const srj_column* t = side ? r : l;
+    const int32_t n     = side ? nr : nl;
+    rows[side]          = t[0].size;
+    for (int32_t c = 0; c < n; ++c)
+      if (t[c].size < 0 || t[c].size != rows[side]) { set_error("%s: the %s key columns have differing or negative row counts", what, side ? "right" : "left"); return SRJ_EINVAL; }
+  }
+  *empty = rows[0] == 0 || rows[1] == 0;
+  if (*empty) return SRJ_OK;
+  for (int side = 0; side < 2; ++side) {
+    const srj_column* t = side ? r : l;
+    for (int32_t c = 0; c < (side ? nr : nl); ++c)
+      if (t[c].type_id != SRJ_STRING && type_width(t[c].type_id) == 0) { set_error("%s: key type %d is not supported", what, t[c].type_id); return SRJ_EUNSUPPORTED; }
+  }
+  if (nl != nr) { set_error("%s: Mismatch in number of columns to be joined on", what); return SRJ_EINVAL; }
+  if (nl > SRJ_MAX_JOIN_KEYS) { set_error("%s: more than %d key columns", what, SRJ_MAX_JOIN_KEYS); return SRJ_EUNSUPPORTED; }
+  for (int32_t c = 0; c < nl; ++c)
+    if (l[c].type_id != r[c].type_id || l[c].scale != r[c].scale) { set_error("%s: Mismatch in joining column data types", what); return SRJ_EINVAL; }
+  if (rows[0] > INT32_MAX || rows[1] > INT32_MAX) { set_error("%s: more than INT32_MAX rows", what); return SRJ_EINVAL; }
+  for (int side = 0; side < 2; ++side) {
+    const srj_column* t = side ? r : l;
+    for (int32_t c = 0; c < nl; ++c) {
+      const char* name = side ? "right key column" : "left key column";
+      const int rc     = t[c].type_id == SRJ_STRING ? check_offsets(what, name, t[c], c) : check_data(what, name, t[c], c);
+      if (rc != SRJ_OK) return rc;
+      if (!aligned_to(t[c].null_mask, 4)) { set_error("%s: %s %d has a null mask not 4-byte aligned", what, name, c); return SRJ_EINVAL; }
+    }
+  }
+  return SRJ_OK;
+}
+
+int64_t srj_hash_join_workspace_bytes(int64_t left_rows, int64_t right_rows)
+{
+  return hash_join_workspace_bytes(std::max<int64_t>(0, left_rows), std::max<int64_t>(0, right_rows));
+}
+
+int srj_hash_inner_join_size(const srj_column* left_keys, int32_t num_left_keys, const srj_column* right_keys, int32_t num_right_keys,
+                             int32_t nulls_equal, int64_t* num_pairs, void* workspace, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "hash_inner_join_size";
+  if (!num_pairs) { set_error("%s: bad argument", what); return SRJ_EINVAL; }
+  int64_t rows[2];
+  bool empty  = false;
+  const int rc = join_check(what, left_keys, num_left_keys, right_keys, num_right_keys, rows, &empty);
+  if (rc != SRJ_OK) return rc;
+  *num_pairs = 0;
+  if (empty) return SRJ_OK;
+  if (!workspace) { set_error("%s: the workspace is needed (srj_hash_join_workspace_bytes)", what); return SRJ_EINVAL; }
+  return launch_hash_join_size(left_keys, right_keys, num_left_keys, rows[0], rows[1], nulls_equal != 0, num_pairs, workspace,
+                               static_cast<cudaStream_t>(stream));
+}
+
+int srj_hash_inner_join(const srj_column* left_keys, int32_t num_left_keys, const srj_column* right_keys, int32_t num_right_keys,
+                        int32_t nulls_equal, int32_t* left_map, int32_t* right_map, void* workspace, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "hash_inner_join";
+  int64_t rows[2];
+  bool empty  = false;
+  int rc = join_check(what, left_keys, num_left_keys, right_keys, num_right_keys, rows, &empty);
+  if (rc != SRJ_OK || empty) return rc;
+  (void)nulls_equal;   // the size call's counts already hold it
+  if ((rc = check_out(what, "workspace", workspace, 1)) != SRJ_OK || (rc = check_out(what, "left map", left_map, 4)) != SRJ_OK ||
+      (rc = check_out(what, "right map", right_map, 4)) != SRJ_OK)
+    return rc;
+  return launch_hash_join(left_keys, right_keys, num_left_keys, rows[0], rows[1], left_map, right_map, workspace, static_cast<cudaStream_t>(stream));
+}
+
+// a gather map of map_len entries (4-byte aligned; NULL only when empty) over a table of table_rows rows
+static int join_check_map(const char* what, const int32_t* map, int64_t map_len, int64_t table_rows)
+{
+  if (map_len < 0 || table_rows < 0) { set_error("%s: Table sizes must be non-negative", what); return SRJ_EINVAL; }
+  if (table_rows > INT32_MAX) { set_error("%s: more than INT32_MAX table rows", what); return SRJ_EINVAL; }
+  return check_out(what, "gather map", map, 4, map_len > 0);
+}
+
+int64_t srj_join_mask_workspace_bytes(int64_t table_rows) { return join_mask_workspace_bytes(std::max<int64_t>(0, table_rows)); }
+
+int srj_join_mark(const int32_t* map, int64_t map_len, int64_t table_rows, void* workspace, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "join_mark";
+  int rc           = join_check_map(what, map, map_len, table_rows);
+  if (rc != SRJ_OK || (rc = check_out(what, "workspace", workspace, 8)) != SRJ_OK) return rc;
+  return launch_join_mark(map, map_len, table_rows, workspace, static_cast<cudaStream_t>(stream));
+}
+
+int srj_join_matched_counts(const void* const* workspaces, int32_t count, int64_t* matched, void* stream)
+{
+  SRJ_API_RANGE();
+  if (count < 0 || (count > 0 && (!workspaces || !matched))) { set_error("join_matched_counts: bad argument"); return SRJ_EINVAL; }
+  for (int32_t i = 0; i < count; ++i)
+    if (!workspaces[i]) { set_error("join_matched_counts: workspace %d is null", i); return SRJ_EINVAL; }
+  if (count == 0) return SRJ_OK;
+  return read_join_matched(workspaces, count, matched, static_cast<cudaStream_t>(stream));
+}
+
+int srj_join_compact(const void* workspace, int64_t table_rows, int32_t matched, int32_t* out, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "join_compact";
+  int rc           = join_check_map(what, nullptr, 0, table_rows);
+  if (rc != SRJ_OK || table_rows == 0) return rc;
+  if ((rc = check_out(what, "workspace", workspace, 1)) != SRJ_OK || (rc = check_out(what, "output", out, 4)) != SRJ_OK) return rc;
+  return launch_join_compact(workspace, table_rows, matched != 0, out, static_cast<cudaStream_t>(stream));
+}
+
+// join_primitives.cu:358-461
+int srj_join_make_outer(const int32_t* left_map, const int32_t* right_map, int64_t map_len, int64_t left_rows, int64_t right_rows,
+                        const void* left_ws, int64_t left_unmatched, const void* right_ws, int64_t right_unmatched, int32_t* out_left,
+                        int32_t* out_right, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "join_make_outer";
+  int rc           = join_check_map(what, left_map, map_len, left_rows);
+  if (rc != SRJ_OK || (rc = join_check_map(what, right_map, map_len, right_rows)) != SRJ_OK) return rc;
+  const bool full = right_ws != nullptr;
+  if (left_unmatched < 0 || left_unmatched > left_rows || (full && (right_unmatched < 0 || right_unmatched > right_rows))) {
+    set_error("%s: unmatched counts outside the table sizes", what);
+    return SRJ_EINVAL;
+  }
+  const int64_t total = map_len + left_unmatched + (full ? right_unmatched : 0);
+  if (total == 0) return SRJ_OK;
+  if ((rc = check_out(what, "left workspace", left_ws, 1)) != SRJ_OK || (rc = check_out(what, "left output", out_left, 4)) != SRJ_OK ||
+      (rc = check_out(what, "right output", out_right, 4)) != SRJ_OK)
+    return rc;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (map_len > 0) {
+    SRJ_CUDA_TRY(cudaMemcpyAsync(out_left, left_map, static_cast<size_t>(map_len) * 4, cudaMemcpyDeviceToDevice, s));
+    SRJ_CUDA_TRY(cudaMemcpyAsync(out_right, right_map, static_cast<size_t>(map_len) * 4, cudaMemcpyDeviceToDevice, s));
+  }
+  if (left_unmatched > 0) {
+    if ((rc = launch_join_compact(left_ws, left_rows, false, out_left + map_len, s)) != SRJ_OK) return rc;
+    if ((rc = launch_join_fill(out_right + map_len, left_unmatched, INT32_MIN, s)) != SRJ_OK) return rc;
+  }
+  if (full && right_unmatched > 0) {
+    const int64_t at = map_len + left_unmatched;
+    if ((rc = launch_join_compact(right_ws, right_rows, false, out_right + at, s)) != SRJ_OK) return rc;
+    if ((rc = launch_join_fill(out_left + at, right_unmatched, INT32_MIN, s)) != SRJ_OK) return rc;
+  }
+  return SRJ_OK;
+}
+
+// join_primitives.cu:549-576
+int srj_join_matched_rows(const int32_t* map, int64_t map_len, int64_t table_rows, uint8_t* out, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "join_matched_rows";
+  int rc           = join_check_map(what, map, map_len, table_rows);
+  if (rc != SRJ_OK || table_rows == 0) return rc;
+  if ((rc = check_out(what, "output", out, 1)) != SRJ_OK) return rc;
+  return launch_join_matched_rows(map, map_len, table_rows, out, static_cast<cudaStream_t>(stream));
+}
+
+}  // extern "C"

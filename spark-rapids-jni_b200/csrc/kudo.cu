@@ -19,6 +19,7 @@
 #include <algorithm>
 #include <vector>
 
+#include "check.hpp"
 #include "common.cuh"
 #include "kernels.hpp"
 
@@ -327,21 +328,6 @@ __global__ void __launch_bounds__(256) kudo_assemble_kernel(const uint8_t* __res
 }
 
 // ---- host side -------------------------------------------------------------------------------------------------------------
-static int kudo_elem_size(int32_t t)
-{
-  switch (t) {
-    case SRJ_INT8: case SRJ_UINT8: case SRJ_BOOL8: return 1;
-    case SRJ_INT16: case SRJ_UINT16: return 2;
-    case SRJ_INT32: case SRJ_UINT32: case SRJ_FLOAT32: case SRJ_TIMESTAMP_DAYS: case SRJ_DURATION_DAYS: case SRJ_DECIMAL32: return 4;
-    case SRJ_INT64: case SRJ_UINT64: case SRJ_FLOAT64: case SRJ_TIMESTAMP_SECONDS: case SRJ_TIMESTAMP_MILLISECONDS:
-    case SRJ_TIMESTAMP_MICROSECONDS: case SRJ_TIMESTAMP_NANOSECONDS: case SRJ_DURATION_SECONDS: case SRJ_DURATION_MILLISECONDS:
-    case SRJ_DURATION_MICROSECONDS: case SRJ_DURATION_NANOSECONDS: case SRJ_DECIMAL64: return 8;
-    case SRJ_DECIMAL128: return 16;
-    case SRJ_STRING: return 0;
-    default: return -1;
-  }
-}
-
 // workspace: [KCol x 256 | sizes int32 x 256 | scols int32 x 256 | bad flag (64 B) | KPartInfo x P | row_base int64 x (P + 1) | chars_base int64 x nstr x (P + 1)]
 struct KudoWs {
   KCol* cols;
@@ -371,7 +357,7 @@ static KudoWs kudo_ws(void* workspace, int P)
   k.chars_base = reinterpret_cast<int64_t*>(w);
   return k;
 }
-int64_t kudo_workspace_bytes(int32_t ncols, int32_t P)
+static int64_t kudo_workspace_bytes(int32_t ncols, int32_t P)
 {
   return static_cast<int64_t>(kKudoMaxCols) * (sizeof(KCol) + 8) + 64 + static_cast<int64_t>(P) * sizeof(KPartInfo) + 64 +
          (static_cast<int64_t>(P) + 1) * 8 + 64 + static_cast<int64_t>(std::max(ncols, 1)) * (static_cast<int64_t>(P) + 1) * 8 + 256;
@@ -384,8 +370,8 @@ static int kudo_upload(const srj_column* cols, int32_t ncols, const KudoWs& ws, 
   int32_t sizes[kKudoMaxCols], scols[kKudoMaxCols];
   int nstr = 0;
   for (int c = 0; c < ncols; ++c) {
-    const int sz = kudo_elem_size(cols[c].type_id);
-    if (sz < 0) return SRJ_EUNSUPPORTED;
+    const int sz = type_width(cols[c].type_id);   // STRING: 0
+    if (sz == 0 && cols[c].type_id != SRJ_STRING) return SRJ_EUNSUPPORTED;
     h[c].data    = static_cast<uint8_t*>(cols[c].data);
     h[c].mask    = reinterpret_cast<uint8_t*>(cols[c].null_mask);
     h[c].offsets = cols[c].offsets;
@@ -401,7 +387,7 @@ static int kudo_upload(const srj_column* cols, int32_t ncols, const KudoWs& ws, 
   return SRJ_OK;
 }
 
-int launch_kudo_split_sizes(const srj_column* cols, int32_t ncols, int64_t num_rows, const int32_t* d_splits, int32_t P, int64_t* d_part_offsets,
+static int launch_kudo_split_sizes(const srj_column* cols, int32_t ncols, int64_t num_rows, const int32_t* d_splits, int32_t P, int64_t* d_part_offsets,
                             int64_t* h_total, void* workspace, cudaStream_t stream)
 {
   const KudoWs ws = kudo_ws(workspace, P);
@@ -419,7 +405,7 @@ int launch_kudo_split_sizes(const srj_column* cols, int32_t ncols, int64_t num_r
   return (bad & 2) ? SRJ_EINVAL : bad ? SRJ_EOVERFLOW : SRJ_OK;
 }
 
-int launch_kudo_split(const srj_column* cols, int32_t ncols, const int32_t* d_splits, int32_t P, const int64_t* d_part_offsets, uint8_t* out,
+static int launch_kudo_split(const srj_column* cols, int32_t ncols, const int32_t* d_splits, int32_t P, const int64_t* d_part_offsets, uint8_t* out,
                       void* workspace, cudaStream_t stream)
 {
   const KudoWs ws = kudo_ws(workspace, P);
@@ -431,7 +417,7 @@ int launch_kudo_split(const srj_column* cols, int32_t ncols, const int32_t* d_sp
   return SRJ_OK;
 }
 
-int launch_kudo_assemble_sizes(const uint8_t* buf, const int64_t* d_part_offsets, int32_t P, const int32_t* type_ids, int32_t ncols, int64_t* h_rows,
+static int launch_kudo_assemble_sizes(const uint8_t* buf, const int64_t* d_part_offsets, int32_t P, const int32_t* type_ids, int32_t ncols, int64_t* h_rows,
                                int64_t* h_char_totals, void* workspace, cudaStream_t stream)
 {
   const KudoWs ws = kudo_ws(workspace, P);
@@ -439,8 +425,8 @@ int launch_kudo_assemble_sizes(const uint8_t* buf, const int64_t* d_part_offsets
   int32_t sizes[kKudoMaxCols], scols[kKudoMaxCols];
   int nstr = 0;
   for (int c = 0; c < ncols; ++c) {
-    sizes[c] = kudo_elem_size(type_ids[c]);
-    if (sizes[c] < 0) return SRJ_EUNSUPPORTED;
+    sizes[c] = type_width(type_ids[c]);   // STRING: 0
+    if (sizes[c] == 0 && type_ids[c] != SRJ_STRING) return SRJ_EUNSUPPORTED;
     if (sizes[c] == 0) scols[nstr++] = c;
     h_char_totals[c] = 0;
   }
@@ -463,7 +449,7 @@ int launch_kudo_assemble_sizes(const uint8_t* buf, const int64_t* d_part_offsets
   return SRJ_OK;
 }
 
-int launch_kudo_assemble(const uint8_t* buf, const int64_t* d_part_offsets, int32_t P, const srj_column* out, int32_t ncols, int64_t total_rows,
+static int launch_kudo_assemble(const uint8_t* buf, const int64_t* d_part_offsets, int32_t P, const srj_column* out, int32_t ncols, int64_t total_rows,
                          void* workspace, cudaStream_t stream)
 {
   const KudoWs ws = kudo_ws(workspace, P);
@@ -480,3 +466,77 @@ int launch_kudo_assemble(const uint8_t* buf, const int64_t* d_part_offsets, int3
 }
 
 }  // namespace srj
+
+// ---- C ABI (include/srj_b200.h) ----
+using namespace srj;
+
+extern "C" {
+
+int64_t srj_kudo_workspace_bytes(int32_t num_columns, int32_t num_partitions) { return kudo_workspace_bytes(std::max(num_columns, 0), std::max(num_partitions, 0)); }
+
+static int kudo_check(const char* what, int32_t ncols, int32_t P, const void* a, const void* b, const void* ws)
+{
+  if (ncols <= 0 || P < 0 || !a || !b || !ws) { set_error("%s: bad argument", what); return SRJ_EINVAL; }
+  if (ncols > 256 || P > 65535) { set_error("%s: at most 256 columns and 65535 partitions", what); return SRJ_EUNSUPPORTED; }
+  return SRJ_OK;
+}
+
+int srj_kudo_split_sizes(const srj_column* cols, int32_t num_columns, int64_t num_rows, const int32_t* d_splits, int32_t num_partitions,
+                         int64_t* d_partition_offsets, int64_t* total_bytes, void* workspace, void* stream)
+{
+  SRJ_API_RANGE();
+  int rc = kudo_check("kudo_split_sizes", num_columns, num_partitions, cols, d_partition_offsets, workspace);
+  if (rc != SRJ_OK) return rc;
+  if (!d_splits || !total_bytes || num_rows < 0 || num_rows > INT32_MAX) { set_error("kudo_split_sizes: bad argument"); return SRJ_EINVAL; }
+  if ((rc = check_rows("kudo_split_sizes", cols, num_columns, num_rows)) != SRJ_OK) return rc;
+  rc = launch_kudo_split_sizes(cols, num_columns, num_rows, d_splits, num_partitions, d_partition_offsets, total_bytes, workspace,
+                               static_cast<cudaStream_t>(stream));
+  if (rc == SRJ_EUNSUPPORTED) set_error("kudo_split_sizes: only fixed-width, decimal and STRING columns");
+  else if (rc == SRJ_EINVAL) set_error("kudo_split_sizes: the splits must lie in [0, %lld]", static_cast<long long>(num_rows));
+  else if (rc == SRJ_EOVERFLOW) set_error("kudo_split_sizes: a partition exceeds the 32-bit section lengths of the Kudo header, or the splits are not increasing");
+  return rc;
+}
+
+int srj_kudo_split(const srj_column* cols, int32_t num_columns, int64_t num_rows, const int32_t* d_splits, int32_t num_partitions,
+                   const int64_t* d_partition_offsets, uint8_t* out, void* workspace, void* stream)
+{
+  SRJ_API_RANGE();
+  int rc = kudo_check("kudo_split", num_columns, num_partitions, cols, d_partition_offsets, workspace);
+  if (rc != SRJ_OK) return rc;
+  if (!d_splits) { set_error("kudo_split: bad argument"); return SRJ_EINVAL; }
+  if ((rc = check_out("kudo_split", "output", out, 4, num_partitions > 0)) != SRJ_OK) return rc;
+  if (num_partitions == 0) return SRJ_OK;
+  (void)num_rows;
+  rc = launch_kudo_split(cols, num_columns, d_splits, num_partitions, d_partition_offsets, out, workspace, static_cast<cudaStream_t>(stream));
+  if (rc == SRJ_EUNSUPPORTED) set_error("kudo_split: only fixed-width, decimal and STRING columns");
+  return rc;
+}
+
+int srj_kudo_assemble_sizes(const uint8_t* partitions, const int64_t* d_partition_offsets, int32_t num_partitions, const int32_t* type_ids,
+                            int32_t num_columns, int64_t* total_rows, int64_t* char_totals, void* workspace, void* stream)
+{
+  SRJ_API_RANGE();
+  int rc = kudo_check("kudo_assemble_sizes", num_columns, num_partitions, type_ids, d_partition_offsets, workspace);
+  if (rc != SRJ_OK) return rc;
+  if ((num_partitions > 0 && !partitions) || !total_rows || !char_totals) { set_error("kudo_assemble_sizes: bad argument"); return SRJ_EINVAL; }
+  rc = launch_kudo_assemble_sizes(partitions, d_partition_offsets, num_partitions, type_ids, num_columns, total_rows, char_totals, workspace,
+                                  static_cast<cudaStream_t>(stream));
+  if (rc == SRJ_EINVAL) set_error("kudo_assemble_sizes: a partition does not start with a Kudo header of %d columns", num_columns);
+  else if (rc == SRJ_EUNSUPPORTED) set_error("kudo_assemble_sizes: only fixed-width, decimal and STRING columns");
+  else if (rc == SRJ_OK && *total_rows > INT32_MAX) { set_error("kudo_assemble_sizes: %lld rows exceed a column", static_cast<long long>(*total_rows)); return SRJ_EOVERFLOW; }
+  return rc;
+}
+
+int srj_kudo_assemble(const uint8_t* partitions, const int64_t* d_partition_offsets, int32_t num_partitions, const srj_column* out,
+                      int32_t num_columns, int64_t total_rows, void* workspace, void* stream)
+{
+  SRJ_API_RANGE();
+  int rc = kudo_check("kudo_assemble", num_columns, num_partitions, out, d_partition_offsets, workspace);
+  if (rc != SRJ_OK) return rc;
+  if ((rc = check_rows("kudo_assemble", out, num_columns, total_rows)) != SRJ_OK) return rc;
+  rc = launch_kudo_assemble(partitions, d_partition_offsets, num_partitions, out, num_columns, total_rows, workspace, static_cast<cudaStream_t>(stream));
+  if (rc == SRJ_EUNSUPPORTED) set_error("kudo_assemble: only fixed-width, decimal and STRING columns");
+  return rc;
+}
+
+}  // extern "C"

@@ -19,6 +19,7 @@
 //                       gather_map (a mask is n / 8 bytes: L2-resident); chars: a warp per 32 destination rows, lane = byte.
 #include <algorithm>
 
+#include "check.hpp"
 #include "common.cuh"
 #include "kernels.hpp"
 
@@ -258,7 +259,7 @@ static int32_t part_tile_rows(int32_t P)
 }
 
 // workspace: [local_pos: n ints | histogram matrix + scan partials (later: the string scans' partials)]
-int64_t partition_workspace_bytes(int64_t num_rows, int32_t P)
+static int64_t partition_workspace_bytes(int64_t num_rows, int32_t P)
 {
   if (num_rows <= 0 || P <= 0) return 256;
   const int64_t ntiles = (num_rows + part_tile_rows(P) - 1) / part_tile_rows(P);
@@ -267,7 +268,7 @@ int64_t partition_workspace_bytes(int64_t num_rows, int32_t P)
   return ((num_rows + tail) * 4 + 255) & ~int64_t{255};
 }
 
-int launch_partition_plan(int32_t* d_ids /* in: hashes, out: partition ids */, int64_t num_rows, int32_t P, int32_t* d_part_offsets,
+static int launch_partition_plan(int32_t* d_ids /* in: hashes, out: partition ids */, int64_t num_rows, int32_t P, int32_t* d_part_offsets,
                           int32_t* d_scatter_map, int32_t* d_gather_map, void* workspace, cudaStream_t stream)
 {
   if (P <= 0 || P > kPartMaxP || num_rows < 0 || num_rows > INT32_MAX) return SRJ_EINVAL;
@@ -509,7 +510,7 @@ __global__ void __launch_bounds__(kPartThreads) partition_move_tile_kernel(const
 // local_pos as written by part_rank_kernel is an ABSOLUTE position (tile start + rank inside the tile); every column
 // (data of fixed-width columns, null masks of all) of `in` moves to `out`.  Returns SRJ_EUNSUPPORTED when the plan's
 // tiles do not fit the staging buffers (more than 1024 partitions): the caller then uses the per-row kernels.
-int launch_partition_move_tiles(const srj_column* in, const srj_column* out, const int* elem_size, int32_t ncols, int64_t n, int32_t P,
+static int launch_partition_move_tiles(const srj_column* in, const srj_column* out, const int* elem_size, int32_t ncols, int64_t n, int32_t P,
                                 const int32_t* d_scatter_map, const void* workspace, unsigned long long* d_null_counts, cudaStream_t stream)
 {
   const int32_t tile = part_tile_rows(P);
@@ -547,7 +548,7 @@ static unsigned grid_for(int64_t n, int per_block)
   return static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>((n + per_block - 1) / per_block, int64_t{sm_count()} * 16)));
 }
 
-int launch_partition_scatter_fixed(const void* in, void* out, int elem_size, const int32_t* d_scatter_map, int64_t n, cudaStream_t stream)
+static int launch_partition_scatter_fixed(const void* in, void* out, int elem_size, const int32_t* d_scatter_map, int64_t n, cudaStream_t stream)
 {
   if (n == 0) return SRJ_OK;
   const unsigned g = grid_for(n, 256);
@@ -563,7 +564,7 @@ int launch_partition_scatter_fixed(const void* in, void* out, int elem_size, con
   return SRJ_OK;
 }
 
-int launch_partition_gather_mask(const uint32_t* in, uint32_t* out, const int32_t* d_gather_map, int64_t n, unsigned long long* d_null_count,
+static int launch_partition_gather_mask(const uint32_t* in, uint32_t* out, const int32_t* d_gather_map, int64_t n, unsigned long long* d_null_count,
                                  cudaStream_t stream)
 {
   if (n == 0) return SRJ_OK;
@@ -573,7 +574,7 @@ int launch_partition_gather_mask(const uint32_t* in, uint32_t* out, const int32_
 }
 
 // out_off[0 .. n] <- offsets of the partitioned column; *d_total (device int32, = out_off[n]) the chars it needs
-int launch_partition_string_offsets(const int32_t* in_off, int32_t* out_off, const int32_t* d_gather_map, int64_t n, void* scan_ws,
+static int launch_partition_string_offsets(const int32_t* in_off, int32_t* out_off, const int32_t* d_gather_map, int64_t n, void* scan_ws,
                                     cudaStream_t stream)
 {
   if (n == 0) {
@@ -585,7 +586,7 @@ int launch_partition_string_offsets(const int32_t* in_off, int32_t* out_off, con
   return launch_i32_exclusive_scan(out_off, n, static_cast<int32_t*>(scan_ws), out_off + n, stream);
 }
 
-int launch_partition_gather_chars(const uint8_t* in_chars, const int32_t* in_off, uint8_t* out_chars, const int32_t* out_off,
+static int launch_partition_gather_chars(const uint8_t* in_chars, const int32_t* in_off, uint8_t* out_chars, const int32_t* out_off,
                                   const int32_t* d_gather_map, int64_t n, cudaStream_t stream)
 {
   if (n == 0) return SRJ_OK;
@@ -595,3 +596,112 @@ int launch_partition_gather_chars(const uint8_t* in_chars, const int32_t* in_off
 }
 
 }  // namespace srj
+
+// ---- C ABI (include/srj_b200.h) ----
+using namespace srj;
+
+extern "C" {
+
+int64_t srj_partition_workspace_bytes(int64_t num_rows, int32_t num_partitions)
+{
+  return partition_workspace_bytes(num_rows, num_partitions);
+}
+
+int srj_partition_plan(int32_t* d_partition_ids, int64_t num_rows, int32_t num_partitions, int32_t* d_partition_offsets,
+                       int32_t* d_scatter_map, int32_t* d_gather_map, void* workspace, void* stream)
+{
+  SRJ_API_RANGE();
+  if (num_rows < 0 || num_partitions <= 0 || !d_partition_offsets || (num_rows > 0 && (!d_partition_ids || !workspace))) {
+    set_error("partition_plan: bad argument");
+    return SRJ_EINVAL;
+  }
+  if (num_rows > INT32_MAX || num_partitions > (1 << 14)) {
+    set_error("partition_plan: %lld rows / %d partitions exceed the int32 row index / 16384 partitions", static_cast<long long>(num_rows), num_partitions);
+    return SRJ_EUNSUPPORTED;
+  }
+  return launch_partition_plan(d_partition_ids, num_rows, num_partitions, d_partition_offsets, d_scatter_map, d_gather_map, workspace,
+                               static_cast<cudaStream_t>(stream));
+}
+
+int srj_hash_partition(const srj_column* keys, int32_t num_keys, int64_t num_rows, uint32_t seed, int32_t num_partitions,
+                       int32_t* d_partition_ids, int32_t* d_partition_offsets, int32_t* d_scatter_map, int32_t* d_gather_map,
+                       void* workspace, void* stream)
+{
+  SRJ_API_RANGE();
+  if (num_keys <= 0 || !keys) { set_error("hash_partition: no key columns"); return SRJ_EINVAL; }
+  if (num_rows > 0 && !d_partition_ids) { set_error("hash_partition: bad argument"); return SRJ_EINVAL; }
+  // the partition count is checked before the keys are hashed: a refused call launches nothing
+  if (num_partitions <= 0) { set_error("hash_partition: %d partitions", num_partitions); return SRJ_EINVAL; }
+  if (num_partitions > (1 << 14)) { set_error("hash_partition: %d partitions exceed 16384 partitions", num_partitions); return SRJ_EUNSUPPORTED; }
+  // the hashes go where the ids will be: part_ids_kernel turns them into ids in place
+  int rc = hash_columns(SRJ_HASH_MURMUR3_32, keys, num_keys, num_rows, seed, d_partition_ids, static_cast<cudaStream_t>(stream));
+  if (rc != SRJ_OK) return rc;
+  return srj_partition_plan(d_partition_ids, num_rows, num_partitions, d_partition_offsets, d_scatter_map, d_gather_map, workspace, stream);
+}
+
+int srj_partition_columns(const srj_column* in, const srj_column* out, int32_t num_columns, int64_t num_rows, int32_t num_partitions,
+                          const int32_t* d_scatter_map, const int32_t* d_gather_map, int64_t* d_null_counts, void* workspace, void* stream)
+{
+  SRJ_API_RANGE();
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (num_columns < 0 || num_rows < 0 || num_partitions <= 0 || (num_columns > 0 && (!in || !out))) { set_error("partition_columns: bad argument"); return SRJ_EINVAL; }
+  if (num_rows > 0 && (!d_scatter_map || !d_gather_map || !workspace)) { set_error("partition_columns: the maps and the plan's workspace are needed"); return SRJ_EINVAL; }
+  if (d_null_counts && num_columns > 0) SRJ_CUDA_TRY(cudaMemsetAsync(d_null_counts, 0, sizeof(int64_t) * num_columns, st));
+  std::vector<int> esz(static_cast<size_t>(num_columns), 0);
+  for (int32_t c = 0; c < num_columns; ++c) {
+    const srj_column& a = in[c];
+    const srj_column& b = out[c];
+    if (a.type_id != b.type_id || a.size != num_rows || b.size != num_rows) { set_error("partition_columns: column %d: type / size mismatch", c); return SRJ_EINVAL; }
+    if (a.type_id == SRJ_STRING) {
+      if (!a.offsets || !b.offsets) { set_error("partition_columns: STRING column %d needs offsets", c); return SRJ_EINVAL; }
+    } else {
+      esz[c] = type_width(a.type_id);
+      if (esz[c] <= 0) { set_error("partition_columns: column %d: unsupported type %d", c, a.type_id); return SRJ_EUNSUPPORTED; }
+      if (num_rows > 0 && (!a.data || !b.data)) { set_error("partition_columns: column %d: NULL data", c); return SRJ_EINVAL; }
+    }
+    if (a.null_mask && !b.null_mask) { set_error("partition_columns: column %d has a null mask but its output has none", c); return SRJ_EINVAL; }
+    if (!a.null_mask && b.null_mask && num_rows > 0) SRJ_CUDA_TRY(cudaMemsetAsync(b.null_mask, 0xff, static_cast<size_t>((num_rows + 31) / 32) * 4, st));
+  }
+  // fixed-width data and every null mask: tile by tile, staged in destination order (plans of <= 1024 partitions) ...
+  int rc = launch_partition_move_tiles(in, out, esz.data(), num_columns, num_rows, num_partitions, d_scatter_map, workspace,
+                                       reinterpret_cast<unsigned long long*>(d_null_counts), st);
+  if (rc == SRJ_EUNSUPPORTED) {
+    // ... or row by row
+    rc = SRJ_OK;
+    for (int32_t c = 0; c < num_columns && rc == SRJ_OK && num_rows > 0; ++c) {
+      if (esz[c] > 0) rc = launch_partition_scatter_fixed(in[c].data, out[c].data, esz[c], d_scatter_map, num_rows, st);
+      if (rc == SRJ_OK && in[c].null_mask)
+        rc = launch_partition_gather_mask(in[c].null_mask, out[c].null_mask, d_gather_map, num_rows,
+                                          d_null_counts ? reinterpret_cast<unsigned long long*>(d_null_counts + c) : nullptr, st);
+    }
+  }
+  if (rc != SRJ_OK) return rc;
+  // STRING columns: the output offsets (lengths through the gather map, then a scan; partials behind the plan's tile order)
+  for (int32_t c = 0; c < num_columns; ++c) {
+    if (in[c].type_id != SRJ_STRING) continue;
+    if (num_rows == 0) {
+      SRJ_CUDA_TRY(cudaMemsetAsync(out[c].offsets, 0, 4, st));   // an empty STRING column still has its offsets[0] = 0
+      continue;
+    }
+    rc = launch_partition_string_offsets(in[c].offsets, out[c].offsets, d_gather_map, num_rows, static_cast<int32_t*>(workspace) + num_rows, st);
+    if (rc != SRJ_OK) return rc;
+  }
+  return SRJ_OK;
+}
+
+int srj_partition_strings(const srj_column* in, const srj_column* out, int32_t num_columns, int64_t num_rows, const int32_t* d_gather_map,
+                          void* stream)
+{
+  SRJ_API_RANGE();
+  if (num_columns < 0 || num_rows < 0 || (num_columns > 0 && (!in || !out))) { set_error("partition_strings: bad argument"); return SRJ_EINVAL; }
+  for (int32_t c = 0; c < num_columns; ++c) {
+    if (in[c].type_id != SRJ_STRING || num_rows == 0) continue;
+    if (!out[c].offsets || !in[c].offsets) { set_error("partition_strings: column %d: NULL offsets", c); return SRJ_EINVAL; }
+    const int rc = launch_partition_gather_chars(static_cast<const uint8_t*>(in[c].data), in[c].offsets, static_cast<uint8_t*>(out[c].data),
+                                                 out[c].offsets, d_gather_map, num_rows, static_cast<cudaStream_t>(stream));
+    if (rc != SRJ_OK) return rc;
+  }
+  return SRJ_OK;
+}
+
+}  // extern "C"

@@ -6,6 +6,7 @@
 // registers.  The rounds are fully unrolled over a rolling 16-word schedule window; round constants live in __constant__
 // (one c[][] operand per round).  SHA-224 / SHA-384 are the SHA-256 / SHA-512 kernels with other initial values and a
 // truncated digest.  A null row (mask bit clear) gets no chars: its output offsets are equal (purge_nonempty_nulls).
+#include "check.hpp"
 #include "common.cuh"
 #include "kernels.hpp"
 
@@ -250,7 +251,7 @@ __global__ void __launch_bounds__(kShaThreads) sha2_offsets_kernel(const uint32_
 
 }  // namespace
 
-int32_t sha2_hex_width(int32_t digest_bits)
+static int32_t sha2_hex_width(int32_t digest_bits)
 {
   switch (digest_bits) {
     case 224: return 56;
@@ -262,13 +263,13 @@ int32_t sha2_hex_width(int32_t digest_bits)
 }
 
 // [rank: words + 1 ints | scan sums]
-int64_t sha2_workspace_bytes(int64_t n)
+static int64_t sha2_workspace_bytes(int64_t n)
 {
   const int64_t words = (n + 31) / 32;
   return 4 * (words + 1 + i32_scan_nchunks(words));
 }
 
-int launch_sha2_sizes(int32_t digest_bits, const srj_column& in, int32_t* d_offsets, int64_t* h_total, void* workspace, cudaStream_t stream)
+static int launch_sha2_sizes(int32_t digest_bits, const srj_column& in, int32_t* d_offsets, int64_t* h_total, void* workspace, cudaStream_t stream)
 {
   const int64_t n     = in.size;
   const int32_t width = sha2_hex_width(digest_bits);
@@ -296,7 +297,7 @@ int launch_sha2_sizes(int32_t digest_bits, const srj_column& in, int32_t* d_offs
   return SRJ_OK;
 }
 
-int launch_sha2(int32_t digest_bits, const srj_column& in, const srj_column& out, cudaStream_t stream)
+static int launch_sha2(int32_t digest_bits, const srj_column& in, const srj_column& out, cudaStream_t stream)
 {
   const int64_t n = in.size;
   if (n == 0) return SRJ_OK;
@@ -319,3 +320,47 @@ int launch_sha2(int32_t digest_bits, const srj_column& in, const srj_column& out
 }
 
 }  // namespace srj
+
+// ---- C ABI (include/srj_b200.h) ----
+using namespace srj;
+
+extern "C" {
+
+int64_t srj_sha2_workspace_bytes(int64_t num_rows) { return sha2_workspace_bytes(std::max<int64_t>(0, num_rows)); }
+
+static int sha2_check(const char* what, int32_t digest_bits, const srj_column* in)
+{
+  if (sha2_hex_width(digest_bits) == 0) { set_error("%s: digest_bits %d is not one of 224, 256, 384, 512", what, digest_bits); return SRJ_EINVAL; }
+  if (!in) { set_error("%s: input is null", what); return SRJ_EINVAL; }
+  if (in->type_id != SRJ_STRING) { set_error("%s: SHA-2 hashing requires a string column (type id %d)", what, in->type_id); return SRJ_EUNSUPPORTED; }
+  if (in->size < 0 || in->size > INT32_MAX) { set_error("%s: %lld rows", what, static_cast<long long>(in->size)); return SRJ_EINVAL; }
+  if (in->size > 0 && !in->offsets) { set_error("%s: the STRING column has no offsets", what); return SRJ_EINVAL; }
+  return SRJ_OK;
+}
+
+int srj_sha2_sizes(int32_t digest_bits, const srj_column* input, int32_t* d_out_offsets, int64_t* total_chars, void* workspace, void* stream)
+{
+  SRJ_API_RANGE();
+  int rc = sha2_check("sha2_sizes", digest_bits, input);
+  if (rc != SRJ_OK) return rc;
+  if (!d_out_offsets || !total_chars) { set_error("sha2_sizes: bad argument"); return SRJ_EINVAL; }
+  if (input->null_mask && input->size > 0 && !workspace) { set_error("sha2_sizes: an input with a null mask needs the workspace (srj_sha2_workspace_bytes)"); return SRJ_EINVAL; }
+  rc = launch_sha2_sizes(digest_bits, *input, d_out_offsets, total_chars, workspace, static_cast<cudaStream_t>(stream));
+  if (rc == SRJ_EOVERFLOW)
+    set_error("sha2_sizes: %lld chars of SHA-%d hex exceed one STRING column (INT32_MAX): hash fewer rows per call", static_cast<long long>(*total_chars), digest_bits);
+  return rc;
+}
+
+int srj_sha2_hash(int32_t digest_bits, const srj_column* input, const srj_column* out, void* stream)
+{
+  SRJ_API_RANGE();
+  int rc = sha2_check("sha2_hash", digest_bits, input);
+  if (rc != SRJ_OK) return rc;
+  if (!out || out->size != input->size || (input->size > 0 && !out->offsets)) { set_error("sha2_hash: the output needs the offsets of srj_sha2_sizes and the input's row count"); return SRJ_EINVAL; }
+  const bool nulls = input->null_mask && input->size > 0;
+  if ((rc = check_out("sha2_hash", "output mask", out->null_mask, 1, nulls)) != SRJ_OK) return rc;
+  if ((rc = check_out("sha2_hash", "output chars", out->data, 16, !input->null_mask && input->size > 0)) != SRJ_OK) return rc;
+  return launch_sha2(digest_bits, *input, *out, static_cast<cudaStream_t>(stream));
+}
+
+}  // extern "C"

@@ -678,7 +678,7 @@ static size_t strings_wide_smem_bytes(int nstr, int stage_bytes, int wpt)
 
 // Can the fast gather serve this schema?  (Host-side, per plan: phase 1 and phase 2 must agree on the offsets
 // protocol.)
-bool strings_wide_eligible(const srj_plan* plan)
+static bool strings_wide_eligible(const srj_plan* plan)
 {
   const int nstr = plan->num_string_columns;
   return nstr >= 8 && nstr <= kSwMaxWpt * kSwMaxCpw;

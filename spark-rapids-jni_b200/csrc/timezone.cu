@@ -15,6 +15,7 @@
 // each mask word from a ballot and the block adds its valid rows to one counter.
 // orc_tz_kernel: the grid-stride map again, both tables staged in shared memory when they fit.
 #include "civil_date.cuh"
+#include "check.hpp"
 #include "common.cuh"
 #include "kernels.hpp"
 #include "map_rows.cuh"
@@ -267,7 +268,8 @@ int launch_convert_unit(const srj_column& in, void* out, const int64_t* inst, co
 
 }  // namespace
 
-int launch_timezone_convert(bool to_utc, const srj_column& in, const srj_column& fixed, const srj_column& dst, int32_t tz_index, void* out,
+// reads the zone's bounds back (one synchronisation), checks it has an entry and 0 or 12 rule integers, then launches
+static int launch_timezone_convert(bool to_utc, const srj_column& in, const srj_column& fixed, const srj_column& dst, int32_t tz_index, void* out,
                             uint32_t* out_mask, cudaStream_t stream)
 {
   if (in.size == 0) return SRJ_OK;
@@ -294,7 +296,8 @@ int launch_timezone_convert(bool to_utc, const srj_column& in, const srj_column&
   return to_utc ? launch_convert_unit<true>(in, out, inst, off, count, rl, stream) : launch_convert_unit<false>(in, out, inst, off, count, rl, stream);
 }
 
-int launch_timezone_convert_multi(const srj_column* in, const srj_column& fixed, const srj_column& dst, int64_t* out, uint32_t* out_mask,
+// in[0..5]: seconds, micros, invalid, tz type, tz offset, tz indices.  Writes out, out_mask and *null_count (one read-back).
+static int launch_timezone_convert_multi(const srj_column* in, const srj_column& fixed, const srj_column& dst, int64_t* out, uint32_t* out_mask,
                                   int64_t* null_count, cudaStream_t stream)
 {
   const int64_t n = in[0].size;
@@ -319,7 +322,8 @@ int launch_timezone_convert_multi(const srj_column* in, const srj_column& fixed,
   return SRJ_OK;
 }
 
-int launch_orc_convert_timezones(const srj_column& in, const int64_t* wt, const int32_t* wo, int32_t wn, int32_t wraw, const int64_t* rt,
+// a table of 0 transitions is a fixed offset (its pointers may be NULL)
+static int launch_orc_convert_timezones(const srj_column& in, const int64_t* wt, const int32_t* wo, int32_t wn, int32_t wraw, const int64_t* rt,
                                  const int32_t* ro, int32_t rn, int32_t rraw, void* out, uint32_t* out_mask, cudaStream_t stream)
 {
   if (in.size == 0) return SRJ_OK;
@@ -334,4 +338,132 @@ int launch_orc_convert_timezones(const srj_column& in, const int64_t* wt, const 
   return SRJ_OK;
 }
 
+int tz_check_flat(const char* what, const char* name, const srj_column* c, int32_t t, int32_t t2, int64_t rows)
+{
+  if (!c) { set_error("%s: the %s column is null", what, name); return SRJ_EINVAL; }
+  if (c->type_id != t && c->type_id != t2) { set_error("%s: the %s column has type id %d", what, name, c->type_id); return SRJ_EINVAL; }
+  if (c->size != rows) { set_error("%s: the %s column has %lld rows, not %lld", what, name, static_cast<long long>(c->size), static_cast<long long>(rows)); return SRJ_EINVAL; }
+  return check_data(what, name, *c);
+}
+
+// the two columns of a time zone table (GpuTimeZoneDB.loadData's layout)
+int tz_check_table(const char* what, const srj_column* fixed, const srj_column* dst)
+{
+  if (!fixed || !dst) { set_error("%s: the time zone table is null", what); return SRJ_EINVAL; }
+  if (fixed->type_id != SRJ_LIST || dst->type_id != SRJ_LIST || fixed->num_children < 1 || !fixed->children || dst->num_children < 1 || !dst->children) {
+    set_error("%s: the time zone table must be LIST<STRUCT<INT64, INT64, INT32>> and LIST<INT32>", what);
+    return SRJ_EINVAL;
+  }
+  if (fixed->size < 0 || fixed->size > INT32_MAX || dst->size != fixed->size) { set_error("%s: the time zone table's columns have mismatched row counts", what); return SRJ_EINVAL; }
+  int rc = check_offsets(what, "transitions' list", *fixed);
+  if (rc == SRJ_OK) rc = check_offsets(what, "DST rules' list", *dst);
+  if (rc != SRJ_OK) return rc;
+  const srj_column* s = &fixed->children[0];
+  if (s->type_id != SRJ_STRUCT || s->num_children != 3 || !s->children) { set_error("%s: the transitions must be STRUCT<INT64, INT64, INT32>", what); return SRJ_EINVAL; }
+  static const char* const names[3] = {"utcInstant", "localInstant", "offset"};
+  for (int i = 0; i < 3; ++i) {
+    rc = tz_check_flat(what, names[i], &s->children[i], i < 2 ? SRJ_INT64 : SRJ_INT32, -1, s->size);
+    if (rc != SRJ_OK) return rc;
+  }
+  return tz_check_flat(what, "DST rules", &dst->children[0], SRJ_INT32, -1, dst->children[0].size);
+}
+
 }  // namespace srj
+
+// ---- C ABI (include/srj_b200.h) ----
+using namespace srj;
+
+extern "C" {
+
+static bool is_timestamp_64(int32_t t) { return t >= SRJ_TIMESTAMP_SECONDS && t <= SRJ_TIMESTAMP_NANOSECONDS; }
+
+// an input of type t with rows > 0 needs its data and out at 8 bytes, and out_mask when it has a mask
+static int tz_check_io(const char* what, const srj_column* in, const void* out, const uint32_t* out_mask)
+{
+  if (in->size < 0) { set_error("%s: bad row count", what); return SRJ_EINVAL; }
+  if (in->size == 0) return SRJ_OK;
+  int rc = check_data(what, "input", *in);
+  if (rc == SRJ_OK) rc = check_out(what, "output", out, 8);
+  if (rc == SRJ_OK) rc = check_out_mask(what, in->null_mask || out_mask, out_mask);   // a mask given is written
+  return rc;
+}
+
+// timezones.cu:80-111, 494-539
+int srj_timezone_convert(int32_t direction, const srj_column* input, const srj_column* fixed_transitions, const srj_column* dst_rules,
+                         int32_t tz_index, void* out, uint32_t* out_mask, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "timezone_convert";
+  if (!input) { set_error("%s: bad argument", what); return SRJ_EINVAL; }
+  if (direction != SRJ_TIMEZONE_TO_UTC && direction != SRJ_TIMEZONE_FROM_UTC) { set_error("%s: unknown direction %d", what, direction); return SRJ_EINVAL; }
+  if (!is_timestamp_64(input->type_id)) { set_error("%s: Unsupported timestamp unit for timezone conversion (type id %d)", what, input->type_id); return SRJ_EUNSUPPORTED; }
+  int rc = tz_check_table(what, fixed_transitions, dst_rules);
+  if (rc != SRJ_OK) return rc;
+  if (tz_index < 0 || tz_index >= fixed_transitions->size) {
+    set_error("%s: time zone index %d is outside the table of %lld zones", what, tz_index, static_cast<long long>(fixed_transitions->size));
+    return SRJ_EINVAL;
+  }
+  if ((rc = tz_check_io(what, input, out, out_mask)) != SRJ_OK) return rc;
+  return launch_timezone_convert(direction == SRJ_TIMEZONE_TO_UTC, *input, *fixed_transitions, *dst_rules, tz_index, out, out_mask,
+                                 static_cast<cudaStream_t>(stream));
+}
+
+// timezones.cu:186-240
+int srj_timezone_convert_multi(const srj_column* seconds, const srj_column* micros, const srj_column* invalid, const srj_column* tz_type,
+                               const srj_column* tz_offset, const srj_column* fixed_transitions, const srj_column* dst_rules,
+                               const srj_column* tz_indices, int64_t* out, uint32_t* out_mask, int64_t* null_count, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "timezone_convert_multi";
+  if (!seconds || !null_count) { set_error("%s: bad argument", what); return SRJ_EINVAL; }
+  if (seconds->type_id != SRJ_INT64) { set_error("%s: seconds column must be of type INT64", what); return SRJ_EUNSUPPORTED; }
+  if (micros && micros->type_id != SRJ_INT32) { set_error("%s: microseconds column must be of type INT32", what); return SRJ_EUNSUPPORTED; }
+  const int64_t n = seconds->size;
+  if (n < 0) { set_error("%s: bad row count", what); return SRJ_EINVAL; }
+  int rc = tz_check_table(what, fixed_transitions, dst_rules);
+  if (rc != SRJ_OK) return rc;
+  const srj_column* cols[6] = {seconds, micros, invalid, tz_type, tz_offset, tz_indices};
+  static const char* const names[6] = {"seconds", "microseconds", "invalid", "tz type", "tz offset", "tz indices"};
+  static const int32_t types[6][2] = {{SRJ_INT64, -1}, {SRJ_INT32, -1}, {SRJ_BOOL8, SRJ_UINT8}, {SRJ_UINT8, -1}, {SRJ_INT32, -1}, {SRJ_INT32, -1}};
+  for (int i = 0; i < 6; ++i)
+    if ((rc = tz_check_flat(what, names[i], cols[i], types[i][0], types[i][1], n)) != SRJ_OK) return rc;
+  if (n == 0) {
+    *null_count = 0;
+    return SRJ_OK;
+  }
+  if ((rc = check_out(what, "output", out, 8)) != SRJ_OK || (rc = check_out_mask(what, true, out_mask)) != SRJ_OK) return rc;
+  const srj_column in[6] = {*seconds, *micros, *invalid, *tz_type, *tz_offset, *tz_indices};
+  return launch_timezone_convert_multi(in, *fixed_transitions, *dst_rules, out, out_mask, null_count, static_cast<cudaStream_t>(stream));
+}
+
+// timezones.cu:380-486; a NULL table is a fixed offset
+int srj_orc_convert_timezones(const srj_column* input, const srj_column* writer_transitions, const srj_column* writer_offsets,
+                              int32_t writer_raw_offset, const srj_column* reader_transitions, const srj_column* reader_offsets,
+                              int32_t reader_raw_offset, void* out, uint32_t* out_mask, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "orc_convert_timezones";
+  if (!input) { set_error("%s: bad argument", what); return SRJ_EINVAL; }
+  if (input->type_id != SRJ_TIMESTAMP_MICROSECONDS) { set_error("%s: Input column must be of type TIMESTAMP_MICROSECONDS", what); return SRJ_EUNSUPPORTED; }
+  const srj_column* tr[2] = {writer_transitions, reader_transitions};
+  const srj_column* of[2] = {writer_offsets, reader_offsets};
+  int32_t rows[2]         = {0, 0};
+  for (int i = 0; i < 2; ++i) {
+    const char* side = i ? "reader" : "writer";
+    if (!tr[i] && !of[i]) continue;
+    if (!tr[i] || !of[i]) { set_error("%s: the %s table needs both its transitions and its offsets", what, side); return SRJ_EINVAL; }
+    if (tr[i]->size < 0 || tr[i]->size > INT32_MAX) { set_error("%s: bad %s table size", what, side); return SRJ_EINVAL; }
+    int rc = tz_check_flat(what, i ? "reader transitions" : "writer transitions", tr[i], SRJ_INT64, -1, tr[i]->size);
+    if (rc == SRJ_OK) rc = tz_check_flat(what, i ? "reader offsets" : "writer offsets", of[i], SRJ_INT32, -1, tr[i]->size);
+    if (rc != SRJ_OK) return rc;
+    rows[i] = static_cast<int32_t>(tr[i]->size);
+  }
+  const int rc = tz_check_io(what, input, out, out_mask);
+  if (rc != SRJ_OK) return rc;
+  auto ptr64 = [&](int i) { return rows[i] ? static_cast<const int64_t*>(tr[i]->data) : nullptr; };
+  auto ptr32 = [&](int i) { return rows[i] ? static_cast<const int32_t*>(of[i]->data) : nullptr; };
+  return launch_orc_convert_timezones(*input, ptr64(0), ptr32(0), rows[0], writer_raw_offset, ptr64(1), ptr32(1), rows[1], reader_raw_offset, out,
+                                      out_mask, static_cast<cudaStream_t>(stream));
+}
+
+}  // extern "C"

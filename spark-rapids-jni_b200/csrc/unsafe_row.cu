@@ -26,6 +26,7 @@
 //   ur_chars_kernel      : chars of every STRING column (a warp per 32 rows, lane = byte)
 #include <algorithm>
 
+#include "check.hpp"
 #include "common.cuh"
 #include "kernels.hpp"
 
@@ -347,7 +348,7 @@ static bool ur_classify(int32_t type_id, int32_t* kind, int32_t* width, int32_t*
   }
 }
 
-int unsafe_row_layout(const int32_t* type_ids, int32_t ncols, int32_t* bitset_bytes, int32_t* fixed_bytes, int32_t* ndec, int32_t* nstr)
+static int unsafe_row_layout(const int32_t* type_ids, int32_t ncols, int32_t* bitset_bytes, int32_t* fixed_bytes, int32_t* ndec, int32_t* nstr)
 {
   if (ncols <= 0 || ncols > kUrMaxCols) return SRJ_EUNSUPPORTED;
   *ndec = *nstr = 0;
@@ -363,7 +364,7 @@ int unsafe_row_layout(const int32_t* type_ids, int32_t ncols, int32_t* bitset_by
 }
 
 // workspace: [UrCol table | 8-byte total | scan partials]
-int64_t unsafe_row_workspace_bytes(int32_t ncols, int64_t n)
+static int64_t unsafe_row_workspace_bytes(int32_t ncols, int64_t n)
 {
   return static_cast<int64_t>(kUrMaxCols) * sizeof(UrCol) + 64 + (i32_scan_nchunks(n + 1) + 64) * 4;
 }
@@ -391,7 +392,7 @@ static int ur_upload(const srj_column* cols, int32_t ncols, void* workspace, UrT
   return SRJ_OK;
 }
 
-int launch_unsafe_row_sizes(const srj_column* cols, int32_t ncols, int64_t n, int32_t* d_row_offsets, void* workspace, int64_t* h_total,
+static int launch_unsafe_row_sizes(const srj_column* cols, int32_t ncols, int64_t n, int32_t* d_row_offsets, void* workspace, int64_t* h_total,
                             cudaStream_t stream)
 {
   UrTable t{};
@@ -417,7 +418,7 @@ int launch_unsafe_row_sizes(const srj_column* cols, int32_t ncols, int64_t n, in
   return launch_i32_exclusive_scan(d_row_offsets, n, sums, d_row_offsets + n, stream);
 }
 
-int launch_unsafe_to_rows(const srj_column* cols, int32_t ncols, int64_t n, const int32_t* d_row_offsets, uint8_t* rows, void* workspace,
+static int launch_unsafe_to_rows(const srj_column* cols, int32_t ncols, int64_t n, const int32_t* d_row_offsets, uint8_t* rows, void* workspace,
                           cudaStream_t stream)
 {
   UrTable t{};
@@ -432,7 +433,7 @@ int launch_unsafe_to_rows(const srj_column* cols, int32_t ncols, int64_t n, cons
   return SRJ_OK;
 }
 
-int launch_unsafe_from_rows(const srj_column* out, int32_t ncols, int64_t n, const uint8_t* rows, const int32_t* d_row_offsets,
+static int launch_unsafe_from_rows(const srj_column* out, int32_t ncols, int64_t n, const uint8_t* rows, const int32_t* d_row_offsets,
                             int64_t* d_null_counts, void* workspace, cudaStream_t stream)
 {
   UrTable t{};
@@ -462,7 +463,7 @@ int launch_unsafe_from_rows(const srj_column* out, int32_t ncols, int64_t n, con
   return SRJ_OK;
 }
 
-int launch_unsafe_from_rows_strings(const srj_column* out, int32_t ncols, int64_t n, const uint8_t* rows, const int32_t* d_row_offsets,
+static int launch_unsafe_from_rows_strings(const srj_column* out, int32_t ncols, int64_t n, const uint8_t* rows, const int32_t* d_row_offsets,
                                     cudaStream_t stream)
 {
   int32_t types[kUrMaxCols];
@@ -483,3 +484,81 @@ int launch_unsafe_from_rows_strings(const srj_column* out, int32_t ncols, int64_
 }
 
 }  // namespace srj
+
+// ---- C ABI (include/srj_b200.h) ----
+using namespace srj;
+
+extern "C" {
+
+int srj_unsafe_row_layout(const int32_t* type_ids, int32_t num_columns, int32_t* bitset_bytes, int32_t* fixed_bytes)
+{
+  if (!type_ids || !bitset_bytes || !fixed_bytes) { set_error("unsafe_row_layout: bad argument"); return SRJ_EINVAL; }
+  int32_t ndec = 0, nstr = 0, fb = 0;
+  const int rc = unsafe_row_layout(type_ids, num_columns, bitset_bytes, &fb, &ndec, &nstr);
+  if (rc != SRJ_OK) { set_error("unsafe_row_layout: 1..256 columns of fixed-width, decimal or STRING type"); return rc; }
+  *fixed_bytes = fb + 16 * ndec;   // every DECIMAL128 field reserves 16 bytes of the variable region
+  return SRJ_OK;
+}
+
+int64_t srj_unsafe_row_workspace_bytes(int32_t num_columns, int64_t num_rows) { return unsafe_row_workspace_bytes(num_columns, std::max<int64_t>(0, num_rows)); }
+
+static int ur_check(const char* what, const srj_column* cols, int32_t ncols, int64_t n, const void* workspace)
+{
+  if (ncols <= 0 || n < 0 || !cols || !workspace) { set_error("%s: bad argument", what); return SRJ_EINVAL; }
+  if (n > INT32_MAX) { set_error("%s: more than INT32_MAX rows", what); return SRJ_EOVERFLOW; }
+  return check_rows(what, cols, ncols, n);
+}
+
+int srj_unsafe_row_sizes(const srj_column* cols, int32_t num_columns, int64_t num_rows, int32_t* d_row_offsets, int64_t* total_bytes,
+                         void* workspace, void* stream)
+{
+  SRJ_API_RANGE();
+  int rc = ur_check("unsafe_row_sizes", cols, num_columns, num_rows, workspace);
+  if (rc != SRJ_OK) return rc;
+  if (!d_row_offsets || !total_bytes) { set_error("unsafe_row_sizes: bad argument"); return SRJ_EINVAL; }
+  rc = launch_unsafe_row_sizes(cols, num_columns, num_rows, d_row_offsets, workspace, total_bytes, static_cast<cudaStream_t>(stream));
+  if (rc == SRJ_EOVERFLOW) set_error("unsafe_row_sizes: %lld bytes of rows exceed one LIST<INT8> column (INT32_MAX): convert fewer rows per call", static_cast<long long>(*total_bytes));
+  else if (rc == SRJ_EUNSUPPORTED) set_error("unsafe_row_sizes: unsupported column type or more than 256 columns");
+  return rc;
+}
+
+int srj_convert_to_unsafe_rows(const srj_column* cols, int32_t num_columns, int64_t num_rows, const int32_t* d_row_offsets, uint8_t* rows,
+                               void* workspace, void* stream)
+{
+  SRJ_API_RANGE();
+  int rc = ur_check("convert_to_unsafe_rows", cols, num_columns, num_rows, workspace);
+  if (rc != SRJ_OK) return rc;
+  if ((rc = check_out("convert_to_unsafe_rows", "rows buffer", rows, 8, num_rows > 0)) != SRJ_OK) return rc;
+  if (!d_row_offsets)
+    for (int32_t c = 0; c < num_columns; ++c)
+      if (cols[c].type_id == SRJ_STRING) { set_error("convert_to_unsafe_rows: STRING columns need the row offsets of srj_unsafe_row_sizes"); return SRJ_EINVAL; }
+  rc = launch_unsafe_to_rows(cols, num_columns, num_rows, d_row_offsets, rows, workspace, static_cast<cudaStream_t>(stream));
+  if (rc == SRJ_EUNSUPPORTED) set_error("convert_to_unsafe_rows: unsupported column type or more than 256 columns");
+  return rc;
+}
+
+int srj_convert_from_unsafe_rows(const uint8_t* rows, const int32_t* d_row_offsets, int64_t num_rows, const srj_column* out, int32_t num_columns,
+                                 int64_t* d_null_counts, void* workspace, void* stream)
+{
+  SRJ_API_RANGE();
+  int rc = ur_check("convert_from_unsafe_rows", out, num_columns, num_rows, workspace);
+  if (rc != SRJ_OK) return rc;
+  if ((rc = check_out("convert_from_unsafe_rows", "rows buffer", rows, 8, num_rows > 0)) != SRJ_OK) return rc;
+  if (!d_row_offsets)
+    for (int32_t c = 0; c < num_columns; ++c)
+      if (out[c].type_id == SRJ_STRING) { set_error("convert_from_unsafe_rows: variable-width rows need their offsets"); return SRJ_EINVAL; }
+  rc = launch_unsafe_from_rows(out, num_columns, num_rows, rows, d_row_offsets, d_null_counts, workspace, static_cast<cudaStream_t>(stream));
+  if (rc == SRJ_EUNSUPPORTED) set_error("convert_from_unsafe_rows: unsupported column type or more than 256 columns");
+  return rc;
+}
+
+int srj_convert_from_unsafe_rows_strings(const uint8_t* rows, const int32_t* d_row_offsets, int64_t num_rows, const srj_column* out,
+                                         int32_t num_columns, void* stream)
+{
+  SRJ_API_RANGE();
+  if (num_columns <= 0 || num_rows < 0 || !out || (num_rows > 0 && (!rows || !d_row_offsets))) { set_error("convert_from_unsafe_rows_strings: bad argument"); return SRJ_EINVAL; }
+  if (check_out("convert_from_unsafe_rows_strings", "rows buffer", rows, 8, false) != SRJ_OK) return SRJ_EINVAL;
+  return launch_unsafe_from_rows_strings(out, num_columns, num_rows, rows, d_row_offsets, static_cast<cudaStream_t>(stream));
+}
+
+}  // extern "C"

@@ -22,6 +22,7 @@
 // AxesToTranspose (inverse undo, then Gray encode), then the transposed coordinates are read out through the same
 // interleave_word with B = numBits.  The N <= 64 coordinates of N * numBits <= 64 bits live in two registers: X[0] and a
 // 64-bit word holding X[1..N-1] at numBits-bit strides, indexed by shifts (no local memory).
+#include "check.hpp"
 #include "common.cuh"
 #include "kernels.hpp"
 
@@ -295,7 +296,8 @@ ZSpread zorder_spread(int32_t n)
 
 }  // namespace
 
-int launch_interleave_bits(const srj_column* cols, int32_t ncols, int64_t rows, int32_t elem_bytes, int32_t* out_offsets, uint8_t* out,
+// out_offsets: rows + 1 int32 (r * ncols * elem_bytes); out: rows * ncols * elem_bytes bytes.  Either may be unaligned.
+static int launch_interleave_bits(const srj_column* cols, int32_t ncols, int64_t rows, int32_t elem_bytes, int32_t* out_offsets, uint8_t* out,
                            cudaStream_t stream)
 {
   if (rows == 0) {
@@ -328,7 +330,7 @@ int launch_interleave_bits(const srj_column* cols, int32_t ncols, int64_t rows, 
   return SRJ_OK;
 }
 
-int launch_hilbert_index(int32_t num_bits, const srj_column* cols, int32_t ncols, int64_t rows, int64_t* out, cudaStream_t stream)
+static int launch_hilbert_index(int32_t num_bits, const srj_column* cols, int32_t ncols, int64_t rows, int64_t* out, cudaStream_t stream)
 {
   if (rows == 0) return SRJ_OK;
   HilbertParams p{};
@@ -343,3 +345,70 @@ int launch_hilbert_index(int32_t num_bits, const srj_column* cols, int32_t ncols
 }
 
 }  // namespace srj
+
+// ---- C ABI (include/srj_b200.h) ----
+using namespace srj;
+
+extern "C" {
+
+// zorder.cu:141-159: at least one column, fixed-width, one type id, the output within INT32_MAX bytes (a logic_error in
+// the reference, so SRJ_EINVAL rather than SRJ_EOVERFLOW).  *elem_bytes = W.
+static int interleave_check(const char* what, const srj_column* cols, int32_t n, int64_t rows, int32_t* elem_bytes)
+{
+  if (n <= 0 || !cols) { set_error("%s: The input table must have at least one column.", what); return SRJ_EINVAL; }
+  if (rows < 0) { set_error("%s: bad row count", what); return SRJ_EINVAL; }
+  const int32_t w = type_width(cols[0].type_id);
+  if (w == 0) { set_error("%s: Only fixed width columns can be used (type id %d)", what, cols[0].type_id); return SRJ_EUNSUPPORTED; }
+  for (int32_t c = 0; c < n; ++c)
+    if (cols[c].type_id != cols[0].type_id) { set_error("%s: All columns of the input table must be the same type.", what); return SRJ_EINVAL; }
+  if (check_rows(what, cols, n, rows) != SRJ_OK) return SRJ_EINVAL;
+  if (rows * static_cast<int64_t>(w) * n > INT32_MAX) { set_error("%s: Input is too large to process", what); return SRJ_EINVAL; }
+  *elem_bytes = w;
+  return SRJ_OK;
+}
+
+int srj_interleave_bits_sizes(const srj_column* cols, int32_t num_columns, int64_t num_rows, int64_t* total_bytes)
+{
+  SRJ_API_RANGE();
+  if (!total_bytes) { set_error("interleave_bits_sizes: bad argument"); return SRJ_EINVAL; }
+  int32_t w    = 0;
+  const int rc = interleave_check("interleave_bits_sizes", cols, num_columns, num_rows, &w);
+  if (rc != SRJ_OK) return rc;
+  *total_bytes = num_rows * w * num_columns;
+  return SRJ_OK;
+}
+
+int srj_interleave_bits(const srj_column* cols, int32_t num_columns, int64_t num_rows, int32_t* out_offsets, uint8_t* out_bytes, void* stream)
+{
+  SRJ_API_RANGE();
+  int32_t w = 0;
+  int rc    = interleave_check("interleave_bits", cols, num_columns, num_rows, &w);
+  if (rc != SRJ_OK) return rc;
+  for (int32_t c = 0; c < num_columns; ++c)
+    if ((rc = check_data("interleave_bits", "column", cols[c], c)) != SRJ_OK) return rc;
+  if ((rc = check_out("interleave_bits", "output offsets", out_offsets, 1)) != SRJ_OK) return rc;
+  if ((rc = check_out("interleave_bits", "output bytes", out_bytes, 1, num_rows > 0)) != SRJ_OK) return rc;
+  return launch_interleave_bits(cols, num_columns, num_rows, w, out_offsets, out_bytes, static_cast<cudaStream_t>(stream));
+}
+
+// zorder.cu:226-237
+int srj_hilbert_index(int32_t num_bits, const srj_column* cols, int32_t num_columns, int64_t num_rows, int64_t* out, void* stream)
+{
+  SRJ_API_RANGE();
+  const char* what = "hilbert_index";
+  if (num_bits <= 0 || num_bits > 32) { set_error("%s: the number of bits must be >0 and <= 32.", what); return SRJ_EINVAL; }
+  if (static_cast<int64_t>(num_bits) * num_columns > 64) { set_error("%s: we only support up to 64 bits of output right now.", what); return SRJ_EINVAL; }
+  if (num_columns <= 0 || !cols) { set_error("%s: at least one column is required.", what); return SRJ_EINVAL; }
+  if (num_rows < 0) { set_error("%s: bad row count", what); return SRJ_EINVAL; }
+  for (int32_t c = 0; c < num_columns; ++c) {
+    if (cols[c].type_id != SRJ_INT32) { set_error("%s: All columns of the input table must be INT32.", what); return SRJ_EUNSUPPORTED; }
+    if (cols[c].size != num_rows) { set_error("%s: column %d has %lld rows, expected %lld", what, c, static_cast<long long>(cols[c].size), static_cast<long long>(num_rows)); return SRJ_EINVAL; }
+  }
+  int rc = SRJ_OK;
+  for (int32_t c = 0; c < num_columns; ++c)
+    if ((rc = check_data(what, "column", cols[c], c)) != SRJ_OK) return rc;
+  if ((rc = check_out(what, "output", out, 1, num_rows > 0)) != SRJ_OK) return rc;
+  return launch_hilbert_index(num_bits, cols, num_columns, num_rows, out, static_cast<cudaStream_t>(stream));
+}
+
+}  // extern "C"

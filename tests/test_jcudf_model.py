@@ -190,7 +190,7 @@ def _const(src, name):
     return m.group(1).strip()
 
 
-def test_planning_constants_match_the_sources():
+def test_planning_constants_and_tile_rule_match_the_sources():
     """The GPU scale tests size their tables from row_plans.py.  If a planner is retuned, they would silently stop
     reaching the cycle points they were written for: fail here instead."""
     capi, fr, frw = _src("capi.cu"), _src("from_rows.cu"), _src("from_rows_wide.cu")
@@ -200,8 +200,9 @@ def test_planning_constants_match_the_sources():
     # srj_plan_create: 64 KB x 3 stages up to 128-byte rows, 100 KB x 2 above; 512-row cap; shrink by 3/4
     assert re.search(r"if \(S <= 128\) \{ tl\.num_stages = 3; tl\.stage_bytes = 64 \* 1024; \}", capi)
     assert re.search(r"else\s+\{ tl\.num_stages = 2; tl\.stage_bytes = 100 \* 1024; \}", capi)
-    assert capi.count("if (R > 512) R = 512;") == 1 and "if (r2 > 512) r2 = 512;" in capi
-    assert "tl.stage_bytes   = (tl.stage_bytes * 3 / 4) & ~127;" in capi
+    # one tile-rounding rule, for the first tile and after every shrink
+    assert capi.count("if (R > 512) R = 512;") == 1 and capi.count("set_tile_rows(tl, S);") == 2
+    assert "tl.stage_bytes = (tl.stage_bytes * 3 / 4) & ~127;" in capi
     assert (P.FR_NARROW_MAX, P.FR_NARROW_STAGE, P.FR_WIDE_STAGE, P.FR_MAX_TILE) == (128, 64 * 1024, 100 * 1024, 512)
     assert int(_const(fr, "kMaxStages")) == P.FR_MAX_STAGES and int(_const(fr, "kStageSlack")) == P.FR_STAGE_SLACK
     assert re.search(r"p\.super_rows\s*=\s*static_cast<int64_t>\(p\.tile_rows\) \* \(row_offsets \? 8 : 2\);", fr)

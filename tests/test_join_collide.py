@@ -1,6 +1,7 @@
 """CPU tests of tests/join_collide.py, the invertible model of the hash join's row hash: the forward model against
 spark_hash_model's Murmur3 where the two definitions agree, every inverse step, the solver on random rows over every
 free-word kind and position, and a guard that ties the model to csrc/join.cu (the null word and the row hash's steps)."""
+import os
 import re
 from collections import namedtuple
 
@@ -180,7 +181,7 @@ def test_tail_collisions_differ_only_in_the_tail():
     assert found >= 8
 
 
-def test_model_matches_join_cu():
+def test_model_matches_join_cu_and_type_width():
     src = JC.join_source()
     assert JC.source_null_key_word(src) == JC.NULL_KEY_WORD
     body = re.search(r"uint32_t row_hash\(.*?\n}\n", src, re.S)
@@ -199,10 +200,12 @@ def test_model_matches_join_cu():
     assert re.search(r"constexpr uint64_t kEmptySlot\s*=\s*~0ull;", src)
     assert re.search(r"while \(4 \* b < 2 \* static_cast<uint64_t>\(right_rows\)\) b <<= 1;", src)
     assert [JC.buckets(n) for n in (0, 1, 2, 3, 1000, 1 << 20)] == [1, 1, 1, 2, 512, 1 << 19]
-    # the widths the model steps by are join_key_width's
+    # the widths the model steps by are type_width's (check.hpp), which join.cu reads its key widths from
+    assert "d.width             = s.type_id == SRJ_STRING ? 0 : type_width(s.type_id);" in src
+    check_hpp = open(os.path.join(os.path.dirname(JC.JOIN_CU), "check.hpp")).read()
     for t, w in JC.WIDTH.items():
         if w:
-            cases = re.search(r"int32_t join_key_width\(int32_t type_id\)\s*{(.*?)\n}", src, re.S).group(1)
+            cases = re.search(r"int type_width\(int32_t type_id\)\s*{(.*?)\n}", check_hpp, re.S).group(1)
             name = {v: k for k, v in vars(SH).items() if k.isupper() and isinstance(v, int) and k not in ("M32", "M64")}[t]
             arm = re.search(r"case SRJ_" + name + r":[^;]*?return (\d+);", cases)
             assert arm and int(arm.group(1)) == w, name

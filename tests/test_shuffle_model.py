@@ -190,10 +190,9 @@ def _const(src, name, file):
     return eval(m.group(1).split("//")[0], {})                       # e.g. 1 << 14
 
 
-def test_shuffle_dispatch_constants_match_the_edge_tests():
+def test_shuffle_dispatch_constants_match_the_edge_tests_in_their_modules():
     part = open(os.path.join(CSRC, "partition.cu")).read()
     kudo = open(os.path.join(CSRC, "kudo.cu")).read()
-    capi = open(os.path.join(CSRC, "capi.cu")).read()
     assert _const(part, "kMoveCols", "partition.cu") == MOVE_COLS
     assert _const(part, "kMoveGroupB", "partition.cu") == MOVE_GROUP_B
     assert _const(part, "kMoveMaxRpt", "partition.cu") == MOVE_MAX_RPT
@@ -205,7 +204,7 @@ def test_shuffle_dispatch_constants_match_the_edge_tests():
     # the tile kernel takes plans whose tile is at most kMoveMaxRpt x 1024 rows; larger plans move row by row
     assert re.search(r"if \(tile > kMoveMaxRpt \* kPartThreads\) return SRJ_EUNSUPPORTED;", part)
     assert part_tile_rows(1024) == MOVE_MAX_RPT * 1024 and part_tile_rows(1025) > MOVE_MAX_RPT * 1024
-    assert re.search(r"num_partitions > \(1 << 14\)", capi) and re.search(r"P > 65535", capi)
+    assert re.search(r"num_partitions > \(1 << 14\)", part) and re.search(r"P > 65535", kudo)
     # the rank kernel's warps: min(32, 51200 / P - 1): 2 warps and 196,608 B of shared memory at P = 16384
     assert re.search(r"\(200 \* 1024\) / \(static_cast<int64_t>\(P\) \* 4\) - 1", part)
     w = max(1, min(32, 51200 // PART_MAX_P - 1))
