@@ -548,6 +548,72 @@ SRJ_API int srj_join_make_outer(const int32_t* left_map, const int32_t* right_ma
                                 int32_t* out_left, int32_t* out_right, void* stream);
 SRJ_API int srj_join_matched_rows(const int32_t* map, int64_t map_len, int64_t table_rows, uint8_t* out, void* stream);
 
+/* ---- Histogram: percentile and median from value-frequency histograms, and createHistogramIfValid ------------------
+ * Reference histogram.cu (Spark's Percentile).  A null_mask counts as nulls here: pass NULL for a column without nulls.
+ *   srj_percentile_workspace_bytes     : bytes of the workspace of the two percentile calls.
+ *   srj_percentile_from_histogram_size : input is LIST<STRUCT<value T, count INT64>> (children[0] the STRUCT, its
+ *                                        children the values and the counts; offsets[0] may be > 0).  T is INT8..INT64,
+ *                                        UINT8..UINT64, FLOAT32, FLOAT64 or BOOL8.  Sorts the rows by length into the
+ *                                        workspace, returns in *valid_rows the rows holding a non-null value (0 when
+ *                                        num_percentages is 0) and in *num_values the doubles of the output (see below);
+ *                                        one stream synchronisation.  The list's own mask is not read: a null list is an
+ *                                        empty one.
+ *   srj_percentile_from_histogram      : with the same arguments and the workspace the size call filled, writes per
+ *                                        valid row and percentage p (in order): the non-null values ordered ascending
+ *                                        (NaN after +inf, every NaN equal, -0.0 before 0.0, BOOL8 nonzero = true), acc
+ *                                        the running sum of their counts, position = (acc.last - 1) * p, lower / higher
+ *                                        = floor / ceil(position); the elements at ranks lower + 1 and higher + 1 are
+ *                                        the first whose acc reaches the rank (the last element when none does); the
+ *                                        result is the lower element when lower == higher or both are equal in T, else
+ *                                        (higher - position) * lo + (position - lower) * hi, each product rounded.
+ *                                        Flat output (output_as_lists 0): out = rows * P doubles, row-major, 0.0 under
+ *                                        null rows; rows doubles, all null, when P is 0 or the rows reference no element
+ *                                        (the reference's early return).  out_mask has one bit per double, each null
+ *                                        where its row is (ceil(num_values / 32) words).  List output: out = valid_rows
+ *                                        * P doubles, out_offsets = rows + 1 (a null row is an empty list), out_mask one
+ *                                        bit per row (ceil(rows / 32) words).  One stream synchronisation (it reads back
+ *                                        the tiers and the list of rows longer than SRJ_HISTOGRAM_CTA_ELEMENTS, at most
+ *                                        16 bytes per SRJ_HISTOGRAM_CTA_ELEMENTS + 1 elements); each such row takes a
+ *                                        radix select with one launch sequence of its own.
+ *   Both: SRJ_EINVAL for an input that is not LIST ("The input column must be of type LIST."), a STRUCT child with
+ *   nulls, not a STRUCT or not of two children, counts with nulls or not INT64 (the reference's messages, in its order);
+ *   SRJ_EOVERFLOW when rows * num_percentages > INT32_MAX; SRJ_EUNSUPPORTED for another T; SRJ_EINVAL for a missing
+ *   or misaligned buffer.  Zero rows touch nothing.  Negative counts give unspecified values.
+ *
+ *   srj_histogram_workspace_bytes      : bytes of the workspace of the two create calls.
+ *   srj_histogram_create_size          : checks the frequencies (INT64, no nulls, the values' size; the reference's
+ *                                        messages) and the values (any fixed-width type, else SRJ_EUNSUPPORTED), then
+ *                                        flags negative and zero frequencies on the device (one stream synchronisation).
+ *                                        A negative one is SRJ_EINVAL ("The input frequencies must not contain negative
+ *                                        values.") and nothing is written.  *out_rows = the output's element rows (the
+ *                                        rows, or for lists the rows with frequency > 0); *value_nulls = the null
+ *                                        values among them.
+ *   srj_histogram_create               : (async) with the same values, frequencies and output_as_lists, and the workspace
+ *                                        the size call filled (its zero flag and keep flags are read on the device).
+ *                                        out_values (*out_rows elements of the values' type) and out_frequencies
+ *                                        (*out_rows INT64) must hold *out_rows elements; when *out_rows > 0 they must be
+ *                                        present, which this call cannot check: the count is on the device.
+ *                                        output_as_lists 0: STRUCT<values, frequencies> of every row; a value is null where
+ *                                        it was or where its frequency is 0, and when some frequency is 0 every null
+ *                                        value's frequency becomes 1; out_values_mask (ceil(rows / 32) words) is needed.
+ *                                        output_as_lists 1: one single-element list per row with frequency > 0, an empty
+ *                                        list for the others (out_offsets rows + 1); the child keeps the values' nulls and
+ *                                        the frequencies; out_values_mask (ceil(*out_rows / 32) words, only those are
+ *                                        written) is needed when the values have a mask.  Zero rows touch nothing.
+ */
+#define SRJ_HISTOGRAM_CTA_ELEMENTS 8192
+SRJ_API int64_t srj_percentile_workspace_bytes(int64_t num_rows, int64_t num_elements, int32_t num_percentages);
+SRJ_API int srj_percentile_from_histogram_size(const srj_column* input, int32_t num_percentages, int32_t output_as_lists, int64_t* valid_rows,
+                                               int64_t* num_values, void* workspace, void* stream);
+SRJ_API int srj_percentile_from_histogram(const srj_column* input, const double* percentages, int32_t num_percentages,
+                                          int32_t output_as_lists, double* out, uint32_t* out_mask, int32_t* out_offsets, void* workspace,
+                                          void* stream);
+SRJ_API int64_t srj_histogram_workspace_bytes(int64_t num_rows);
+SRJ_API int srj_histogram_create_size(const srj_column* values, const srj_column* frequencies, int32_t output_as_lists, int64_t* out_rows,
+                                      int64_t* value_nulls, void* workspace, void* stream);
+SRJ_API int srj_histogram_create(const srj_column* values, const srj_column* frequencies, int32_t output_as_lists, void* out_values,
+                                 uint32_t* out_values_mask, int64_t* out_frequencies, int32_t* out_offsets, void* workspace, void* stream);
+
 /* ---- multi-GPU configuration (SURVEY 8e: row-range shards + one all-gather of per-column chunks) ---------------- */
 /* ---- Spark HashPartitioning on the device (SURVEY 8f rank 1) ---------------------------------------------------
  * The consumer of Hash.murmurHash32: GpuHashPartitioning computes pmod(murmur3_32(42, keys), P) per row and then

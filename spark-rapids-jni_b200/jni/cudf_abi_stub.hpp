@@ -23,7 +23,7 @@ struct device_buffer {
 namespace cudf {
 using size_type     = int32_t;
 using bitmask_type  = uint32_t;
-enum class type_id : int32_t { EMPTY = 0, INT8 = 1, UINT8 = 5, INT32 = 3, INT64 = 4, BOOL8 = 11, TIMESTAMP_DAYS = 12, TIMESTAMP_MICROSECONDS = 15,
+enum class type_id : int32_t { EMPTY = 0, INT8 = 1, UINT8 = 5, INT32 = 3, INT64 = 4, FLOAT64 = 10, BOOL8 = 11, TIMESTAMP_DAYS = 12, TIMESTAMP_MICROSECONDS = 15,
                               STRING = 23, LIST = 24, DECIMAL32 = 25, DECIMAL64 = 26, DECIMAL128 = 27,
                               STRUCT = 28 };
 struct data_type {

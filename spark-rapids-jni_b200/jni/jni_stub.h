@@ -6,6 +6,7 @@
 #define JNICALL
 typedef int32_t jint;
 typedef int64_t jlong;
+typedef double jdouble;
 typedef uint8_t jboolean;
 typedef int32_t jsize;
 class _jobject {};
@@ -15,6 +16,7 @@ typedef jobject jthrowable;
 typedef jobject jarray;
 typedef jarray jintArray;
 typedef jarray jlongArray;
+typedef jarray jdoubleArray;
 typedef jobject jstring;
 struct JNIEnv {
   const char* GetStringUTFChars(jstring, jboolean*);
@@ -27,6 +29,8 @@ struct JNIEnv {
   void ReleaseIntArrayElements(jintArray, jint*, jint);
   jlong* GetLongArrayElements(jlongArray, jboolean*);
   void ReleaseLongArrayElements(jlongArray, jlong*, jint);
+  jdouble* GetDoubleArrayElements(jdoubleArray, jboolean*);
+  void ReleaseDoubleArrayElements(jdoubleArray, jdouble*, jint);
   jlongArray NewLongArray(jsize);
   void SetLongArrayRegion(jlongArray, jsize, jsize, const jlong*);
   jintArray NewIntArray(jsize);

@@ -107,6 +107,16 @@ SYMBOLS = {
     "srj_join_make_outer": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
                                       C.c_void_p, C.c_void_p, C.c_void_p]),
     "srj_join_matched_rows": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]),
+    "srj_percentile_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int64, C.c_int32]),
+    "srj_percentile_from_histogram_size": (C.c_int, [C.POINTER(SrjColumn), C.c_int32, C.c_int32, C.POINTER(C.c_int64),
+                                                     C.POINTER(C.c_int64), C.c_void_p, C.c_void_p]),
+    "srj_percentile_from_histogram": (C.c_int, [C.POINTER(SrjColumn), C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                C.c_void_p, C.c_void_p]),
+    "srj_histogram_workspace_bytes": (C.c_int64, [C.c_int64]),
+    "srj_histogram_create_size": (C.c_int, [C.POINTER(SrjColumn), C.POINTER(SrjColumn), C.c_int32, C.POINTER(C.c_int64), C.POINTER(C.c_int64),
+                                            C.c_void_p, C.c_void_p]),
+    "srj_histogram_create": (C.c_int, [C.POINTER(SrjColumn), C.POINTER(SrjColumn), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p]),
     "srj_partition_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int32]),
     "srj_hash_partition": (C.c_int, [C.POINTER(SrjColumn), C.c_int32, C.c_int64, C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
