@@ -614,6 +614,46 @@ SRJ_API int srj_histogram_create_size(const srj_column* values, const srj_column
 SRJ_API int srj_histogram_create(const srj_column* values, const srj_column* frequencies, int32_t output_as_lists, void* out_values,
                                  uint32_t* out_values_mask, int64_t* out_frequencies, int32_t* out_offsets, void* workspace, void* stream);
 
+/* ---- Arithmetic: Spark's multiply with ANSI / try overflow handling, and round / bround ----------------------------
+ * Reference multiply.cu, round_float.cu and cudf's round/round.cu.  A null_mask counts as nulls here: pass NULL for a
+ * column without nulls.  Both calls set *error_row to -1 first.
+ *   srj_multiply : left * right, each a column or a scalar.  An operand with a scalar validity (a device byte, non-zero =
+ *                  valid, as cudf::scalar::validity_data() holds it) is a scalar: its data is its one device value and its
+ *                  size and mask are not read.  Rows = the column operand's size.  Types INT8, INT16, INT32, INT64, FLOAT32,
+ *                  FLOAT64, the same on both sides.  An integer row overflows when its exact product is outside the type:
+ *                  by default it wraps; with is_try_mode it is null; with is_ansi_mode *error_row is the smallest
+ *                  overflowing row with both operands valid (-1 when none) and the output is not a result.  Floats are IEEE
+ *                  products in every mode.  A row is null when an operand is (a null scalar: every row); a null row holds
+ *                  0.  out: rows elements of the type, aligned to the element.  out_mask: ceil(rows / 32) words, 4-byte
+ *                  aligned, needed when the result can hold nulls (an operand has a mask or is a scalar, or try mode on an
+ *                  integer type), else it may be NULL (when given, it is written).  *null_count: the output's nulls when
+ *                  the result can hold nulls, else 0.  The null count and the error row are read back together (one
+ *                  stream synchronisation) when either is needed; otherwise the call is asynchronous.  Errors, in this
+ *                  order: SRJ_EINVAL for two scalars or differing types, SRJ_EUNSUPPORTED for another type, SRJ_EINVAL for
+ *                  differing row counts (column * column), for is_ansi_mode with is_try_mode, and for a missing or
+ *                  misaligned buffer.
+ *   srj_round    : (async, unless ANSI on an integer type with decimal_places < 0: one stream synchronisation for
+ *                  *error_row) rounds to decimal_places with method SRJ_ROUND_HALF_UP or SRJ_ROUND_HALF_EVEN.  Zero rows
+ *                  return SRJ_OK before any check.  FLOAT32 / FLOAT64: n = T(pow(10, |dp|)); dp == 0: round / rint;
+ *                  dp > 0: modf, then int_part + round(frac * n) / n; dp < 0: round(e / n) * n; each operation rounded
+ *                  to nearest in T.  INT8..INT64: dp >= 0 copies; dp < 0 rounds to a multiple of 10^-dp (HALF_UP away
+ *                  from zero, HALF_EVEN to the even multiple), the exact result wrapped to the type; with is_ansi_mode
+ *                  *error_row is the smallest valid row whose exact result is outside the type.  DECIMAL32 / 64 / 128
+ *                  (ANSI ignored): the output's scale is -dp; the same scale copies; a larger input scale multiplies by
+ *                  10^k, wrapping; a scale movement k above 9 / 18 / 38 digits gives zeros; else the storage integer is
+ *                  rounded and divided by 10^k exactly.  out: rows elements of the input's type, aligned to the element
+ *                  (8 bytes at most).  out_mask (ceil(rows / 32) words, 4-byte aligned) receives a copy of the input's
+ *                  mask, all ones when it has none, and may be NULL only when the input has no mask.  SRJ_EUNSUPPORTED
+ *                  for another type, then SRJ_EINVAL for another method and for a missing or misaligned buffer.
+ */
+#define SRJ_ROUND_HALF_UP 0
+#define SRJ_ROUND_HALF_EVEN 1
+SRJ_API int srj_multiply(const srj_column* left, const uint8_t* left_scalar_valid, const srj_column* right, const uint8_t* right_scalar_valid,
+                         int32_t is_ansi_mode, int32_t is_try_mode, void* out, uint32_t* out_mask, int64_t* null_count, int64_t* error_row,
+                         void* stream);
+SRJ_API int srj_round(const srj_column* input, int32_t decimal_places, int32_t method, int32_t is_ansi_mode, void* out, uint32_t* out_mask,
+                      int64_t* error_row, void* stream);
+
 /* ---- multi-GPU configuration (SURVEY 8e: row-range shards + one all-gather of per-column chunks) ---------------- */
 /* ---- Spark HashPartitioning on the device (SURVEY 8f rank 1) ---------------------------------------------------
  * The consumer of Hash.murmurHash32: GpuHashPartitioning computes pmod(murmur3_32(42, keys), P) per row and then

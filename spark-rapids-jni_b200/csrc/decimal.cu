@@ -333,8 +333,8 @@ Div div_or_one(int k) { return host_div(k < 1 || k > 38 ? 0 : k); }
 
 }  // namespace
 
-// The null counter of the calling host thread on the current device, allocated once.  A call reads its count back before
-// it returns, and one host thread makes one call at a time, so a counter per (thread, device) is never shared by two calls
+// The counters of the calling host thread on the current device (two words: the null count here, and arithmetic.cu's
+// first error row beside its null count), allocated once.  A call reads them back before it returns, and one host thread makes one call at a time, so a counter per (thread, device) is never shared by two calls
 // in flight.
 struct NullCounters {
   std::map<int, unsigned long long*> by_device;
@@ -352,7 +352,7 @@ int null_counter(unsigned long long** out)
   unsigned long long*& p = counters.by_device[dev];
   if (!p) {
     unsigned long long* q = nullptr;
-    SRJ_CUDA_TRY(cudaMalloc(&q, sizeof(*q)));
+    SRJ_CUDA_TRY(cudaMalloc(&q, 2 * sizeof(*q)));
     p = q;
   }
   *out = p;

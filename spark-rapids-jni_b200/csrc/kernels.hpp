@@ -79,8 +79,8 @@ int launch_i32_exclusive_scan(int32_t* v, int64_t n, int32_t* sums, int32_t* tai
 // exclusive scan of v[0 .. n] in place by one CTA (kudo.cu; n up to a few 10^5); v[n] receives the total
 int launch_i64_scan_small(int64_t* v, int n, cudaStream_t stream);
 
-// decimal.cu: a device counter of the calling host thread on the current device, allocated once; a call that uses it
-// reads it back before it returns.
+// decimal.cu: two adjacent device counters of the calling host thread on the current device, allocated once; a call that
+// uses them reads them back before it returns.
 int null_counter(unsigned long long** out);
 
 // timezone.cu: GpuTimeZoneDB.loadData's table (LIST<STRUCT<INT64, INT64, INT32>> transitions, LIST<INT32> rules), and a

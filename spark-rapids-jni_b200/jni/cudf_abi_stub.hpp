@@ -23,7 +23,7 @@ struct device_buffer {
 namespace cudf {
 using size_type     = int32_t;
 using bitmask_type  = uint32_t;
-enum class type_id : int32_t { EMPTY = 0, INT8 = 1, UINT8 = 5, INT32 = 3, INT64 = 4, FLOAT64 = 10, BOOL8 = 11, TIMESTAMP_DAYS = 12, TIMESTAMP_MICROSECONDS = 15,
+enum class type_id : int32_t { EMPTY = 0, INT8 = 1, INT16 = 2, UINT8 = 5, INT32 = 3, INT64 = 4, FLOAT32 = 9, FLOAT64 = 10, BOOL8 = 11, TIMESTAMP_DAYS = 12, TIMESTAMP_MICROSECONDS = 15,
                               STRING = 23, LIST = 24, DECIMAL32 = 25, DECIMAL64 = 26, DECIMAL128 = 27,
                               STRUCT = 28 };
 struct data_type {
@@ -63,6 +63,16 @@ struct lists_column_view {                           // lists/lists_column_view.
   column_view child() const;
   size_type size() const;
 };
+struct scalar {                                      // scalar/scalar.hpp: a device value and a device validity flag
+  data_type type() const;
+  bool const* validity_data() const;
+};
+namespace detail {
+template <typename T>
+struct fixed_width_scalar : scalar {
+  T const* data() const;
+};
+}  // namespace detail
 struct list_scalar {                                 // scalar/scalar.hpp: one row of a LIST column, held by its child
   list_scalar(column&& data, bool is_valid, rmm::cuda_stream_view stream);
   column_view view() const;

@@ -23,6 +23,7 @@ struct JNIEnv {
   void ReleaseStringUTFChars(jstring, const char*);
   jclass FindClass(const char*);
   jint ThrowNew(jclass, const char*);
+  jint Throw(jthrowable);
   jboolean ExceptionCheck();
   jsize GetArrayLength(jarray);
   jint* GetIntArrayElements(jintArray, jboolean*);

@@ -46,6 +46,20 @@ inline void throw_java(JNIEnv* env, const char* cls, const char* msg)
   if (!env->ExceptionCheck()) env->ThrowNew(env->FindClass(cls), msg);
 }
 
+// Throws com.nvidia.spark.rapids.jni.ExceptionWithRowIndex(row) through its (I)V constructor, as the reference's
+// CATCH_EXCEPTION_WITH_ROW_INDEX does, after freeing the call's output buffers: an ANSI row error returns no column.
+inline void throw_row_index(JNIEnv* env, int64_t row, std::vector<rmm::device_buffer*> outputs)
+{
+  for (rmm::device_buffer* b : outputs) *b = rmm::device_buffer{};
+  if (env->ExceptionCheck()) return;
+  jclass cls = env->FindClass("com/nvidia/spark/rapids/jni/ExceptionWithRowIndex");
+  if (!cls) return;
+  jmethodID ctor = env->GetMethodID(cls, "<init>", "(I)V");
+  if (!ctor) return;
+  jobject ex = env->NewObject(cls, ctor, static_cast<jint>(row));
+  if (ex) env->Throw(static_cast<jthrowable>(ex));
+}
+
 // No C++ exception (rmm::out_of_memory, std::bad_alloc, ...) may leave a JNI function: map them to the Java classes.
 // Call from a catch (...) block.
 inline void throw_from_exception(JNIEnv* env)

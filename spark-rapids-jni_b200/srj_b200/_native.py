@@ -117,6 +117,10 @@ SYMBOLS = {
                                             C.c_void_p, C.c_void_p]),
     "srj_histogram_create": (C.c_int, [C.POINTER(SrjColumn), C.POINTER(SrjColumn), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_void_p]),
+    "srj_multiply": (C.c_int, [C.POINTER(SrjColumn), C.c_void_p, C.POINTER(SrjColumn), C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
+                               C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_void_p]),
+    "srj_round": (C.c_int, [C.POINTER(SrjColumn), C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64),
+                            C.c_void_p]),
     "srj_partition_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int32]),
     "srj_hash_partition": (C.c_int, [C.POINTER(SrjColumn), C.c_int32, C.c_int64, C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

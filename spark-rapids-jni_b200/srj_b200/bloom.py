@@ -26,19 +26,65 @@ INT32_MAX = 2**31 - 1
 
 
 class Scalar:
-    """ai.rapids.cudf.Scalar of type LIST<UINT8>: one row holding the bytes of one serialized filter."""
+    """ai.rapids.cudf.Scalar.  Of type LIST<UINT8> (dtype None): one row holding the bytes of one serialized filter.  Of a
+    fixed-width type: `data` holds the value's bytes and `valid` one device byte, non-zero when the scalar is valid, as
+    cudf::scalar holds them on the device (Arithmetic.multiply reads both there)."""
 
-    def __init__(self, data: torch.Tensor):
+    def __init__(self, data: torch.Tensor, dtype: Optional[DType] = None, valid: Optional[torch.Tensor] = None):
         self.data = data
+        self.dtype = dtype
+        self.valid = valid
+
+    _NUMPY = {DType.INT8: "int8", DType.INT16: "int16", DType.INT32: "int32", DType.INT64: "int64", DType.FLOAT32: "float32",
+              DType.FLOAT64: "float64"}
+
+    @staticmethod
+    def _fixed(type_id: int, value, device=None) -> "Scalar":
+        import numpy as np
+        dev = device if device is not None else torch.device("cuda", torch.cuda.current_device())
+        raw = np.array([0 if value is None else value], dtype=Scalar._NUMPY[type_id]).view(np.uint8)
+        return Scalar(torch.from_numpy(raw.copy()).to(dev), DType(type_id),
+                      torch.tensor([value is not None], dtype=torch.uint8, device=dev))
+
+    @staticmethod
+    def fromByte(v, device=None) -> "Scalar":
+        return Scalar._fixed(DType.INT8, v, device)
+
+    @staticmethod
+    def fromShort(v, device=None) -> "Scalar":
+        return Scalar._fixed(DType.INT16, v, device)
+
+    @staticmethod
+    def fromInt(v, device=None) -> "Scalar":
+        return Scalar._fixed(DType.INT32, v, device)
+
+    @staticmethod
+    def fromLong(v, device=None) -> "Scalar":
+        return Scalar._fixed(DType.INT64, v, device)
+
+    @staticmethod
+    def fromFloat(v, device=None) -> "Scalar":
+        return Scalar._fixed(DType.FLOAT32, v, device)
+
+    @staticmethod
+    def fromDouble(v, device=None) -> "Scalar":
+        return Scalar._fixed(DType.FLOAT64, v, device)
+
+    @staticmethod
+    def fromNull(dtype: DType, device=None) -> "Scalar":
+        return Scalar._fixed(dtype.type_id, None, device)
 
     def getType(self) -> DType:
-        return DType(DType.LIST)
+        return DType(DType.LIST) if self.dtype is None else self.dtype
+
+    def isValid(self) -> bool:
+        return self.valid is None or bool(self.valid.item())
 
     def getListAsColumnView(self) -> ColumnView:
         return ColumnView(DType.UINT8, self.data.numel(), self.data, null_count=0)
 
     def close(self):
-        self.data = None
+        self.data = self.valid = None
 
     def __enter__(self):
         return self
