@@ -17,6 +17,7 @@ array of little-endian halves.
 """
 from __future__ import annotations
 
+import math
 from typing import Optional, Tuple
 
 import numpy as np
@@ -82,10 +83,20 @@ def _round_half(x: np.ndarray, mode: int) -> np.ndarray:
     return np.rint(x) if mode == HALF_EVEN else _round_half_up(x)
 
 
+def pow10(k: int) -> float:
+    """The C library's pow(10, k) in double, inf past the double range: the reference computes n = std::pow(10, |dp|) on
+    the host.  That is not always the double nearest 10^k (glibc gives 10^23 one ulp high), and numpy's power need not
+    agree with it (on some CPUs it differs at 10^301), so the oracle calls the same pow."""
+    try:
+        return math.pow(10.0, k)
+    except OverflowError:
+        return math.inf
+
+
 def round_float(e: np.ndarray, dp: int, mode: int) -> np.ndarray:
     t = e.dtype.type
     with np.errstate(all="ignore"):
-        n = t(np.power(np.float64(10.0), abs(int(dp))))
+        n = t(pow10(abs(int(dp))))
         if dp == 0:
             return _round_half(e, mode)
         if dp > 0:

@@ -222,11 +222,16 @@ __device__ __forceinline__ double round_half(double x, bool even) { return even 
 __device__ __forceinline__ float modf_t(float x, float* ip) { return modff(x, ip); }
 __device__ __forceinline__ double modf_t(double x, double* ip) { return modf(x, ip); }
 
-// RN(e / n) for n = RN(10^k) >= 10 or +inf, y = RN(1 / n).  For finite e and n: q0 = RN(e * y) is within 1.5 ulp of e / n,
-// the first correction RN(q0 + (e - q0 n) y) (the remainder exact through the FMA) makes it faithful, and the second is
-// correctly rounded (Markstein's theorem: y within half an ulp of 1 / n, the quotient faithful).  A quotient in the
-// subnormal range is only ever rounded to an integer, where any value below 0.5 in magnitude gives the same +-0.  The
-// sign is e's, as for 0 / n.  e infinite or NaN, or n infinite: e * y is e / n (inf, NaN, or +-0 from y = 0).
+// RN(e / n) for n = pow(10, k) >= 10 or +inf, y = RN(1 / n).  For finite e and n: q0 = RN(e * y) is within 1.5 ulp of
+// e / n, the first correction RN(q0 + (e - q0 n) y) (the remainder exact through the FMA) makes it faithful, and the
+// second is correctly rounded (Markstein's theorem: y within half an ulp of 1 / n, the quotient faithful).  From n > 2^126
+// (float, dp >= 38) or 2^1022 (double, dp >= 308) y is subnormal and carries fewer bits, so the theorem's premise fails;
+// and the dp > 0 branch returns m / n itself (|m| <= n), which is subnormal for m = +-1 (float, dp = 38) and m = +-1, +-2
+// (double, dp = 308).  That the result still equals IEEE e / n there is measured, not proved: test_gpu_round_exhaustive.py
+// checks every float32 input at every dp, and double quotients at the smallest distance from a rounding midpoint that
+// their numerators reach, the subnormal ones included.  The dp < 0 branch rounds its quotient to an integer, where any
+// subnormal gives the same +-0.  The sign is e's, as for 0 / n.  e infinite or NaN, or n infinite: e * y is e / n (inf,
+// NaN, or +-0 from y = 0).
 template <class T>
 __device__ __forceinline__ T div_n(T e, T n, T y)
 {
