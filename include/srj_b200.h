@@ -654,6 +654,30 @@ SRJ_API int srj_multiply(const srj_column* left, const uint8_t* left_scalar_vali
 SRJ_API int srj_round(const srj_column* input, int32_t decimal_places, int32_t method, int32_t is_ansi_mode, void* out, uint32_t* out_mask,
                       int64_t* error_row, void* stream);
 
+/* ---- DecimalUtils.floatingPointToDecimal: Spark's CAST(float / double AS DECIMAL) ----------------------------------
+ * Reference decimal_utils.cu:1174-1417 over cudf's fixed_point/detail/floating_conversion.hpp, bit for bit inside the
+ * domain below, the reference's integer wraps included.  input: FLOAT32 or FLOAT64 (a null_mask counts as nulls);
+ * out_type_id: SRJ_DECIMAL32 / 64 / 128 with `precision` digits at cudf `scale` (the value is out * 10^scale).  A null,
+ * NaN or infinite row is null and holds 0; any other value is scaled and rounded as Spark does (a double rounds half up
+ * after half a unit in the last place is added, a float at the edge of its precision), and a result not strictly inside
+ * (-10^precision, 10^precision) is null, holds 0 and fails.  out: rows elements of the output type, aligned to the
+ * element (8 bytes at most); out_mask: ceil(rows / 32) words, 4-byte aligned, always written; *null_count its nulls.
+ * One stream synchronisation reads back *null_count and *failure_row.
+ * Defined here where the reference is not:
+ *   - *failure_row is the smallest failing row, or -1 (the reference stores some failing row, racing between threads);
+ *   - the domain: precision 1..9 (DECIMAL32), 1..18 (DECIMAL64), 1..38 (DECIMAL128), and scale in [-precision, 38]
+ *     (Spark scale -38 .. precision, the legacy negative scales included), where every power of ten the reference forms
+ *     for the bound and the scale factor fits the type; outside it SRJ_EINVAL before any launch;
+ *   - the reference divides DECIMAL64 rows whose last-digit exponent is 63 by 10^64 mod 2^64 = 0; the quotient is all
+ *     ones here, so those rows (|x| near 2^210 * 10^-scale) fail.
+ * Errors, in this order: SRJ_EINVAL for a NULL input, null_count or failure_row; SRJ_EUNSUPPORTED for an input that is
+ * not FLOAT32 / FLOAT64 or an output type that is not DECIMAL32 / 64 / 128; SRJ_EINVAL for a precision or scale outside
+ * the domain and a negative row count; zero rows return SRJ_OK here, touching nothing; then SRJ_EINVAL for missing or
+ * misaligned input data, output or output mask.
+ */
+SRJ_API int srj_float_to_fixed_point(const srj_column* input, int32_t out_type_id, int32_t precision, int32_t scale, void* out,
+                                     uint32_t* out_mask, int64_t* null_count, int64_t* failure_row, void* stream);
+
 /* ---- multi-GPU configuration (SURVEY 8e: row-range shards + one all-gather of per-column chunks) ---------------- */
 /* ---- Spark HashPartitioning on the device (SURVEY 8f rank 1) ---------------------------------------------------
  * The consumer of Hash.murmurHash32: GpuHashPartitioning computes pmod(murmur3_32(42, keys), P) per row and then

@@ -30,33 +30,12 @@ using dec::u128;
 
 constexpr int kDecThreads = 256;
 constexpr int kDecRows    = 4;
-constexpr int kMaxPow     = 76;
-
-struct PowTable {
-  uint64_t w[kMaxPow + 1][4];   // 10^k in little-endian 64-bit limbs
-};
-
-// 10^0 .. 10^76, each the previous times 10 in 32-bit halves (a constant expression, so one definition serves both copies)
-constexpr PowTable make_pow10()
-{
-  PowTable t{};
-  t.w[0][0] = 1;
-  for (int k = 1; k <= kMaxPow; ++k) {
-    uint64_t carry = 0;
-    for (int i = 0; i < 4; ++i) {
-      const uint64_t lo = (t.w[k - 1][i] & 0xffffffffu) * 10 + carry;
-      const uint64_t hi = (t.w[k - 1][i] >> 32) * 10 + (lo >> 32);
-      t.w[k][i]         = (hi << 32) | (lo & 0xffffffffu);
-      carry             = hi >> 32;
-    }
-  }
-  return t;
-}
+using dec::kMaxPow;
+using dec::PowTable;
+using dec::make_pow10;
 
 __constant__ PowTable c_pow10 = make_pow10();
 constexpr PowTable h_pow10    = make_pow10();
-static_assert(h_pow10.w[19][0] == 10000000000000000000ull && h_pow10.w[20][1] == 5 && h_pow10.w[76][3] == 0x161bcca7119915b5ull,
-              "powers of ten");
 
 U256 host_pow(int k) { return U256{{h_pow10.w[k][0], h_pow10.w[k][1], h_pow10.w[k][2], h_pow10.w[k][3]}}; }
 Div host_div(int k) { return dec::make_div((static_cast<u128>(h_pow10.w[k][1]) << 64) | h_pow10.w[k][0]); }   // k <= 38

@@ -128,6 +128,35 @@ __host__ __device__ __forceinline__ uint64_t reciprocal_word(uint64_t d)
   return v3 - static_cast<uint64_t>(t >> 64) - d;
 }
 
+// 10^0 .. 10^76 in little-endian 64-bit limbs; the low limb of 10^k is also 10^k mod 2^64 (k < 64)
+constexpr int kMaxPow = 76;
+
+struct PowTable {
+  uint64_t w[kMaxPow + 1][4];
+};
+
+// each power the previous times 10 in 32-bit halves (a constant expression, so one definition serves the host and the
+// __constant__ copies of decimal.cu and float_to_decimal.cu)
+constexpr PowTable make_pow10()
+{
+  PowTable t{};
+  t.w[0][0] = 1;
+  for (int k = 1; k <= kMaxPow; ++k) {
+    uint64_t carry = 0;
+    for (int i = 0; i < 4; ++i) {
+      const uint64_t lo = (t.w[k - 1][i] & 0xffffffffu) * 10 + carry;
+      const uint64_t hi = (t.w[k - 1][i] >> 32) * 10 + (lo >> 32);
+      t.w[k][i]         = (hi << 32) | (lo & 0xffffffffu);
+      carry             = hi >> 32;
+    }
+  }
+  return t;
+}
+
+static_assert(make_pow10().w[19][0] == 10000000000000000000ull && make_pow10().w[20][1] == 5 &&
+                make_pow10().w[76][3] == 0x161bcca7119915b5ull,
+              "powers of ten");
+
 // A divisor: D = (d1, d0) = d << s with the top bit set, and its 3-by-2 reciprocal v.  zero: d == 0, which divides as the
 // reference's bit-serial loop does (every quotient bit set, the remainder the dividend's low 128 bits).
 struct Div {
@@ -216,6 +245,20 @@ __host__ __device__ __forceinline__ U256 udivrem(const U256& n, const Div& D, u1
   q.w[0] = div_3by2(static_cast<uint64_t>(r >> 64), static_cast<uint64_t>(r), x0, D, &r);
   *rem = r >> D.s;
   return q;
+}
+
+// n / d for n < 2^128: udivrem's two low quotient limbs (its two high ones are 0), all ones for d == 0 as udivrem
+__host__ __device__ __forceinline__ u128 udiv128(u128 n, const Div& D)
+{
+  if (D.zero) return ~u128(0);
+  const int b        = D.s & 63;
+  const uint64_t n0  = static_cast<uint64_t>(n), n1 = static_cast<uint64_t>(n >> 64);
+  const uint64_t y0  = n0 << b, y1 = shl_in(n1, n0, b), y2 = b ? n1 >> (64 - b) : 0;
+  const bool wide    = D.s >= 64;                                     // (y2, y1) < 2^s <= D: the high limbs are 0
+  u128 r             = wide ? (static_cast<u128>(y2) << 64) | y1 : static_cast<u128>(y2);
+  const uint64_t q1  = div_3by2(static_cast<uint64_t>(r >> 64), static_cast<uint64_t>(r), wide ? y0 : y1, D, &r);
+  const uint64_t q0  = div_3by2(static_cast<uint64_t>(r >> 64), static_cast<uint64_t>(r), wide ? 0 : y0, D, &r);
+  return (static_cast<u128>(q1) << 64) | q0;
 }
 
 // The reference's signed divide (decimal_utils.cu:163-183): quotient truncated toward zero, negated when the signs of n

@@ -2,7 +2,7 @@
 // DecimalUtils.java (reference DecimalUtilsJni.cpp).  Inputs: two cudf::column_view* of DECIMAL128; output: a jlongArray
 // of two heap cudf::column* -- BOOL8 overflow flags and the result (DECIMAL128 at the requested scale, INT64 for an
 // integral divide) -- each with the AND of the input masks and its null count.  floatingPointToDecimal, the sixth
-// native, is not bound.  A null handle throws NullPointerException; C-ABI errors map to the classes of srj_jni_common.hpp.
+// native, is bound in DecimalUtilsCastJni.cpp.  A null handle throws NullPointerException; C-ABI errors map to the classes of srj_jni_common.hpp.
 #include "srj_jni_common.hpp"
 
 using namespace srjshim;

@@ -121,6 +121,8 @@ SYMBOLS = {
                                C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_void_p]),
     "srj_round": (C.c_int, [C.POINTER(SrjColumn), C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64),
                             C.c_void_p]),
+    "srj_float_to_fixed_point": (C.c_int, [C.POINTER(SrjColumn), C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                           C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_void_p]),
     "srj_partition_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int32]),
     "srj_hash_partition": (C.c_int, [C.POINTER(SrjColumn), C.c_int32, C.c_int64, C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

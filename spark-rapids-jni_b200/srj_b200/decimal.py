@@ -8,9 +8,14 @@ can need more than 128 bits.
     t = DecimalUtils.remainder128(a, b, remainderScale)
     t = DecimalUtils.add128(a, b, targetScale) / subtract128(a, b, targetScale)
 
+    r = DecimalUtils.floatingPointToDecimal(x, DType(DType.DECIMAL64, -2), 18)   # CAST(x AS DECIMAL(18, 2))
+    r.result, r.failureRowId                                            # (srj_float_to_fixed_point)
+
 Scales are cudf scales (the value is unscaled * 10^scale).  Both output columns carry the AND of the inputs' null masks
 and its null count.  Java's IllegalArgumentException raises ValueError; errors of the native layer (a column that is not
 DECIMAL128, differing row counts, an unsupported scale combination) raise CudfException; a null column raises TypeError.
+floatingPointToDecimal's result carries a mask only when it has nulls; its failureRowId is the smallest failing row, or
+-1.
 """
 import ctypes as C
 
@@ -56,6 +61,14 @@ def _check_scale_gap(a: ColumnView, b: ColumnView):
         raise ValueError("The intermediate scale for calculating the result exceeds 256-bit representation")
 
 
+class CastFloatToDecimalResult:
+    """DecimalUtils.CastFloatToDecimalResult: the cast's column and the smallest failing row (negative: none)."""
+
+    def __init__(self, result: ColumnVector, failureRowId: int):
+        self.result = result
+        self.failureRowId = failureRowId
+
+
 class DecimalUtils:
     @staticmethod
     def multiply128(a: ColumnView, b: ColumnView, productScale: int, interimCast: bool = True) -> Table:
@@ -89,3 +102,23 @@ class DecimalUtils:
         """a - b at the finer input scale, rounded HALF_UP to targetScale (Spark 3.4+)."""
         _check_scale_gap(a, b)
         return _binary(SUBTRACT, a, b, targetScale, False, "DecimalUtils.subtract128")
+
+    @staticmethod
+    def floatingPointToDecimal(input: ColumnView, outputType: DType, precision: int) -> CastFloatToDecimalResult:
+        """CAST(float / double AS DECIMAL(precision, -outputType.scale)) as Spark computes it: a null, NaN or infinite
+        row is null; a value whose rounded result has more than `precision` digits is null and fails."""
+        what = "DecimalUtils.floatingPointToDecimal"
+        if input is None:
+            raise TypeError(f"{what}: column is null")                                # JNI_NULL_CHECK
+        n = input.size
+        dev = _device(input)
+        with torch.cuda.device(dev):
+            out = _empty(n * max(outputType.size_in_bytes(), 1), torch.uint8, dev)
+            mask = _empty((n + 31) // 32, torch.int32, dev)
+            nulls, failure = C.c_int64(0), C.c_int64(-1)
+            N.check(N.lib().srj_float_to_fixed_point(C.byref(input._c()), outputType.type_id, int(precision), outputType.scale,
+                                                     out.data_ptr() if n else None, mask.data_ptr() if n else None,
+                                                     C.byref(nulls), C.byref(failure), _stream_ptr()), what)
+            col = ColumnVector(DType(outputType.type_id, outputType.scale), n, out, mask if nulls.value else None,
+                               null_count=nulls.value)
+            return CastFloatToDecimalResult(col, failure.value)
