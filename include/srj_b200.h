@@ -678,6 +678,64 @@ SRJ_API int srj_round(const srj_column* input, int32_t decimal_places, int32_t m
 SRJ_API int srj_float_to_fixed_point(const srj_column* input, int32_t out_type_id, int32_t precision, int32_t scale, void* out,
                                      uint32_t* out_mask, int64_t* null_count, int64_t* failure_row, void* stream);
 
+/* ---- NumberConverter and CastStrings' radix casts: Spark's conv(), bin() and hex() ---------------------------------
+ * Reference number_converter.cu (Spark 3.5's NumberConverter), cast_long_to_binary_string.cu, hex.cu and
+ * CastStringJni.cpp's fromIntegersWithBase (cudf's from_integers / integers_to_hex, then the extract ^0?([0-9a-fA-F]+)$).
+ * Every output is a STRING column: d_out_offsets int32[rows + 1] and its chars.  Each op except bytesToHex is a sizes call
+ * (lengths, exclusive scan, one stream synchronisation to read back *total_chars) and a write call (async) taking the
+ * same arguments, the offsets and the workspace the sizes call filled.  A result of more than INT32_MAX chars returns
+ * SRJ_EOVERFLOW from the sizes call (its offsets are then not a column).
+ *
+ *   srj_conv_*         : NumberConverter.convert / isConvertOverflow.  input is a STRING column, or NULL with a scalar
+ *                        string of scalar_len bytes at the device pointer `scalar` (scalar_len < 0: a null scalar,
+ *                        SRJ_EINVAL).  from_base / to_base are INT32 columns, or NULL with the int from / to.  A scalar
+ *                        input needs at least one base column; the output has the column arguments' rows, and base
+ *                        columns of other row counts are SRJ_EINVAL.  A row is null when its input or a base is null,
+ *                        when from is outside [2, 36] or |to| outside [2, 36] (every row when both are scalars), or when
+ *                        the string is empty after trimming ' ' from both ends.  Otherwise an optional '-' and the
+ *                        digits below `from` (0-9, A-Z, a-z) that follow it accumulate in 64 bits; the first other byte
+ *                        ends the number.  On overflow (past 2^64 - 1) the value is all ones.  A negative input with
+ *                        to > 0 is negated (all ones stays); with to < 0 a value with its top bit set is negated and the
+ *                        result gets a '-', as does a negative input.  Digits are upper case, "0" for zero.
+ *                        srj_conv_sizes writes the offsets, out_mask (ceil(rows / 32) words, always) and *null_count;
+ *                        srj_conv writes the chars.  srj_conv_overflow sets *overflow to 1 when a non-null row with valid
+ *                        bases overflows (Spark's ANSI error), else 0; it synchronizes.
+ *   srj_long_to_binary_* : CastStrings.fromLongToBinary.  INT64 only: the 64-bit two's complement in binary without
+ *                        leading zeros, "0" for zero.
+ *   srj_integers_to_string_* : CastStrings.fromIntegersWithBase.  INT8..INT64, UINT8..UINT64.  base 10: decimal with '-'
+ *                        for negative values; base 16: upper-case hex of the value's own width without leading zeros ("0"
+ *                        for zero, INT8 -1 -> "FF").  Another base is SRJ_EINVAL ("Bases supported 10, 16; Actual: N",
+ *                        checked before the type; the JNI shim throws the reference's CastException on row 0).
+ *   srj_bytes_to_hex_* : CastStrings.bytesToHex.  STRING, or LIST<UINT8> read as its child's bytes: each byte becomes two
+ *                        upper-case hex digits.  The offsets are twice the input's, rebased to 0, so a null row keeps its
+ *                        span; its chars hold the hex of its bytes.  No workspace.
+ * For bin, fromIntegersWithBase and bytesToHex the output mask is a copy of the input's: out->null_mask is needed when
+ * the input has a mask and is not written when it has none.  Null rows of bin and fromIntegersWithBase have length 0.
+ * Workspaces: srj_conv_workspace_bytes(rows) (it keeps each row's parsed value), srj_long_to_binary_workspace_bytes and
+ * srj_integers_to_string_workspace_bytes (the scan's), 8-byte aligned.
+ * Defined here where the reference is not: the base-column row check, the chars under null bytesToHex rows, and
+ * SRJ_EOVERFLOW past INT32_MAX chars.  Errors: SRJ_EUNSUPPORTED for another input or base type; SRJ_EINVAL for a NULL or
+ * misaligned buffer, a bad row count or base, and the scalar cases above.
+ */
+SRJ_API int64_t srj_conv_workspace_bytes(int64_t num_rows);
+SRJ_API int srj_conv_sizes(const srj_column* input, const uint8_t* scalar, int32_t scalar_len, const srj_column* from_base, int32_t from,
+                           const srj_column* to_base, int32_t to, int32_t* d_out_offsets, uint32_t* out_mask, int64_t* null_count,
+                           int64_t* total_chars, void* workspace, void* stream);
+SRJ_API int srj_conv(const srj_column* input, const uint8_t* scalar, int32_t scalar_len, const srj_column* from_base, int32_t from,
+                     const srj_column* to_base, int32_t to, const int32_t* d_out_offsets, uint8_t* out_chars, const void* workspace,
+                     void* stream);
+SRJ_API int srj_conv_overflow(const srj_column* input, const uint8_t* scalar, int32_t scalar_len, const srj_column* from_base, int32_t from,
+                              const srj_column* to_base, int32_t to, int32_t* overflow, void* stream);
+SRJ_API int64_t srj_long_to_binary_workspace_bytes(int64_t num_rows);
+SRJ_API int srj_long_to_binary_sizes(const srj_column* input, int32_t* d_out_offsets, int64_t* total_chars, void* workspace, void* stream);
+SRJ_API int srj_long_to_binary(const srj_column* input, const srj_column* out, void* stream);
+SRJ_API int64_t srj_integers_to_string_workspace_bytes(int64_t num_rows);
+SRJ_API int srj_integers_to_string_sizes(const srj_column* input, int32_t base, int32_t* d_out_offsets, int64_t* total_chars, void* workspace,
+                                         void* stream);
+SRJ_API int srj_integers_to_string(const srj_column* input, int32_t base, const srj_column* out, void* stream);
+SRJ_API int srj_bytes_to_hex_sizes(const srj_column* input, int32_t* d_out_offsets, int64_t* total_chars, void* stream);
+SRJ_API int srj_bytes_to_hex(const srj_column* input, const srj_column* out, void* stream);
+
 /* ---- multi-GPU configuration (SURVEY 8e: row-range shards + one all-gather of per-column chunks) ---------------- */
 /* ---- Spark HashPartitioning on the device (SURVEY 8f rank 1) ---------------------------------------------------
  * The consumer of Hash.murmurHash32: GpuHashPartitioning computes pmod(murmur3_32(42, keys), P) per row and then

@@ -14,7 +14,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "srj_b200", "libsrj_b200.so")
-SOURCES = ["capi.cu", "from_rows.cu", "from_rows_wide.cu", "to_rows.cu", "to_rows_var.cu", "strings.cu", "hash.cu", "hash_nested.cu", "sharding.cu", "partition.cu", "unsafe_row.cu", "kudo.cu", "host_api.cu", "sha2.cu", "bloom_filter.cu", "zorder.cu", "iceberg.cu", "decimal.cu", "datetime.cu", "join.cu", "timezone.cu", "cast_datetime.cu", "histogram.cu", "arithmetic.cu", "float_to_decimal.cu"]
+SOURCES = ["capi.cu", "from_rows.cu", "from_rows_wide.cu", "to_rows.cu", "to_rows_var.cu", "strings.cu", "hash.cu", "hash_nested.cu", "sharding.cu", "partition.cu", "unsafe_row.cu", "kudo.cu", "host_api.cu", "sha2.cu", "bloom_filter.cu", "zorder.cu", "iceberg.cu", "decimal.cu", "datetime.cu", "join.cu", "timezone.cu", "cast_datetime.cu", "histogram.cu", "arithmetic.cu", "float_to_decimal.cu", "radix.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

@@ -73,6 +73,11 @@ struct fixed_width_scalar : scalar {
   T const* data() const;
 };
 }  // namespace detail
+struct string_scalar : scalar {                      // scalar/scalar.hpp: the string's bytes on the device
+  char const* data() const;
+  size_type size() const;
+  bool is_valid(rmm::cuda_stream_view stream) const;
+};
 struct list_scalar {                                 // scalar/scalar.hpp: one row of a LIST column, held by its child
   list_scalar(column&& data, bool is_valid, rmm::cuda_stream_view stream);
   column_view view() const;

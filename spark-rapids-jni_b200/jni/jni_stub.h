@@ -38,6 +38,7 @@ struct JNIEnv {
   void SetIntArrayRegion(jintArray, jsize, jsize, const jint*);
   struct _jmethodID* GetMethodID(jclass, const char*, const char*);
   jobject NewObject(jclass, struct _jmethodID*, ...);
+  jstring NewStringUTF(const char*);
 };
 typedef struct _jmethodID* jmethodID;
 #define JNI_ABORT 2

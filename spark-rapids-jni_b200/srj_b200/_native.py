@@ -123,6 +123,21 @@ SYMBOLS = {
                             C.c_void_p]),
     "srj_float_to_fixed_point": (C.c_int, [C.POINTER(SrjColumn), C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                            C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_void_p]),
+    "srj_conv_workspace_bytes": (C.c_int64, [C.c_int64]),
+    "srj_conv_sizes": (C.c_int, [C.POINTER(SrjColumn), C.c_void_p, C.c_int32, C.POINTER(SrjColumn), C.c_int32, C.POINTER(SrjColumn), C.c_int32,
+                                 C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_void_p, C.c_void_p]),
+    "srj_conv": (C.c_int, [C.POINTER(SrjColumn), C.c_void_p, C.c_int32, C.POINTER(SrjColumn), C.c_int32, C.POINTER(SrjColumn), C.c_int32,
+                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "srj_conv_overflow": (C.c_int, [C.POINTER(SrjColumn), C.c_void_p, C.c_int32, C.POINTER(SrjColumn), C.c_int32, C.POINTER(SrjColumn),
+                                    C.c_int32, C.POINTER(C.c_int32), C.c_void_p]),
+    "srj_long_to_binary_workspace_bytes": (C.c_int64, [C.c_int64]),
+    "srj_long_to_binary_sizes": (C.c_int, [C.POINTER(SrjColumn), C.c_void_p, C.POINTER(C.c_int64), C.c_void_p, C.c_void_p]),
+    "srj_long_to_binary": (C.c_int, [C.POINTER(SrjColumn), C.POINTER(SrjColumn), C.c_void_p]),
+    "srj_integers_to_string_workspace_bytes": (C.c_int64, [C.c_int64]),
+    "srj_integers_to_string_sizes": (C.c_int, [C.POINTER(SrjColumn), C.c_int32, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p, C.c_void_p]),
+    "srj_integers_to_string": (C.c_int, [C.POINTER(SrjColumn), C.c_int32, C.POINTER(SrjColumn), C.c_void_p]),
+    "srj_bytes_to_hex_sizes": (C.c_int, [C.POINTER(SrjColumn), C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
+    "srj_bytes_to_hex": (C.c_int, [C.POINTER(SrjColumn), C.POINTER(SrjColumn), C.c_void_p]),
     "srj_partition_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int32]),
     "srj_hash_partition": (C.c_int, [C.POINTER(SrjColumn), C.c_int32, C.c_int64, C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -71,6 +71,14 @@ class Scalar:
         return Scalar._fixed(DType.FLOAT64, v, device)
 
     @staticmethod
+    def fromString(v, device=None) -> "Scalar":
+        """A STRING scalar: `data` holds its UTF-8 bytes (str) or the bytes given, on the device; None is a null scalar."""
+        dev = device if device is not None else torch.device("cuda", torch.cuda.current_device())
+        raw = b"" if v is None else (v.encode() if isinstance(v, str) else bytes(v))
+        return Scalar(torch.tensor(list(raw), dtype=torch.uint8, device=dev), DType(DType.STRING),
+                      torch.tensor([v is not None], dtype=torch.uint8, device=dev))
+
+    @staticmethod
     def fromNull(dtype: DType, device=None) -> "Scalar":
         return Scalar._fixed(dtype.type_id, None, device)
 

@@ -1,12 +1,19 @@
 """com.nvidia.spark.rapids.jni.CastStrings' string-to-timestamp and string-to-date casts (CastStrings.java) over the C ABI
-(include/srj_b200.h: srj_cast_parse_timestamps, srj_cast_parse_dates).
+(include/srj_b200.h: srj_cast_parse_timestamps, srj_cast_parse_dates), and its radix casts (srj_long_to_binary_*,
+srj_integers_to_string_*, srj_bytes_to_hex_*).
 
     tbl = TimeZoneTable.from_zoneinfo(["America/Los_Angeles", "UTC"])
     ts = CastStrings.toTimestamp(strings, "America/Los_Angeles", False, Version(Version.VANILLA_SPARK, 3, 5, 0), tbl)
     dates = CastStrings.toDate(strings, False)
 
 parseTimestampStrings returns the intermediate STRUCT (result, seconds, microseconds, tz type, tz offset, tz index);
-toTimestamp composes it with GpuTimeZoneDB.convertTimestampColumnToUTCWithTzCv.  Under ANSI both casts return None when
+toTimestamp composes it with GpuTimeZoneDB.convertTimestampColumnToUTCWithTzCv.
+
+    b = CastStrings.fromLongToBinary(longs)              # bin(): "1010", 64 digits for a negative value
+    s = CastStrings.fromIntegersWithBase(ints, 16)       # hex() of integers ("FF" for INT8 -1); base 10: decimal
+    h = CastStrings.bytesToHex(strings_or_binary)        # hex() of STRING / LIST<UINT8>: two digits a byte
+
+fromIntegersWithBase with a base other than 10 or 16 raises CastException on row 0, as the reference does.  Under ANSI both casts return None when
 the result has more nulls than the input, as the reference does.  A null argument raises TypeError (NullPointerException),
 an unknown default zone ValueError (IllegalArgumentException), errors of the native layer CudfException.
 """
@@ -68,6 +75,44 @@ def _epoch_day_now(zone: str) -> int:
     z = SHORT_IDS.get(zone, zone)
     tz = _dt.timezone.utc if z in ("Z", "UTC") else zoneinfo.ZoneInfo(z)
     return (_dt.datetime.now(tz).date() - _dt.date(1970, 1, 1)).days
+
+
+class CastException(RuntimeError):
+    """com.nvidia.spark.rapids.jni.CastException: "Error casting data on row <row>: <string>"."""
+
+    def __init__(self, stringWithError: str, rowWithError: int):
+        super().__init__(f"Error casting data on row {rowWithError}: {stringWithError}")
+        self.stringWithError, self.rowWithError = stringWithError, rowWithError
+
+    def getRowWithError(self) -> int:
+        return self.rowWithError
+
+    def getStringWithError(self) -> str:
+        return self.stringWithError
+
+
+def _radix_cast(input: ColumnView, what: str, sizes, write, ws_bytes=None) -> ColumnVector:
+    """sizes -> chars -> write of one radix cast; the result's mask is a copy of the input's"""
+    from .radix import _device as _radix_device, strings_result
+    if input is None:
+        raise TypeError(f"{what}: input column is null")
+    n = input.size
+    dev = _radix_device(input)
+    with torch.cuda.device(dev):
+        stream = _stream_ptr()
+        cin = input._c()
+        offsets = _empty(n + 1, torch.int32, dev)
+        total = C.c_int64(0)
+        if ws_bytes is None:
+            N.check(sizes(C.byref(cin), offsets.data_ptr(), C.byref(total), stream), what)
+        else:
+            ws = _empty(max(ws_bytes(n), 8), torch.uint8, dev)
+            N.check(sizes(C.byref(cin), offsets.data_ptr(), C.byref(total), ws.data_ptr(), stream), what)
+        chars = _empty(total.value, torch.uint8, dev)
+        mask = _empty((n + 31) // 32, torch.int32, dev) if input.mask is not None else None
+        out = strings_result(n, offsets, chars, mask, input.getNullCount())
+        N.check(write(C.byref(cin), C.byref(out._c()), stream), what)
+        return out
 
 
 class CastStrings:
@@ -136,3 +181,30 @@ class CastStrings:
         if ansiEnabled and result.getNullCount() > input.getNullCount():
             return None
         return result
+
+    @staticmethod
+    def fromLongToBinary(cv: ColumnView) -> ColumnVector:
+        """bin(): each INT64 as its 64-bit two's complement in binary without leading zeros ("0" for zero)."""
+        lib = N.lib()
+        return _radix_cast(cv, "CastStrings.fromLongToBinary", lib.srj_long_to_binary_sizes, lib.srj_long_to_binary,
+                           lib.srj_long_to_binary_workspace_bytes)
+
+    @staticmethod
+    def fromIntegersWithBase(cv: ColumnView, base: int) -> ColumnVector:
+        """Integers as strings: base 10 decimal with '-', base 16 upper-case hex of the value's own width without leading
+        zeros.  Any other base raises CastException on row 0."""
+        what = "CastStrings.fromIntegersWithBase"
+        if cv is None:
+            raise TypeError(f"{what}: input column is null")
+        base = int(base)
+        if base not in (10, 16):
+            raise CastException(f"Bases supported 10, 16; Actual: {base}", 0)
+        lib = N.lib()
+        return _radix_cast(cv, what, lambda c, o, t, w, s: lib.srj_integers_to_string_sizes(c, base, o, t, w, s),
+                           lambda c, o, s: lib.srj_integers_to_string(c, base, o, s), lib.srj_integers_to_string_workspace_bytes)
+
+    @staticmethod
+    def bytesToHex(cv: ColumnView) -> ColumnVector:
+        """hex() of STRING or LIST<UINT8> (BinaryType): two upper-case digits a byte."""
+        lib = N.lib()
+        return _radix_cast(cv, "CastStrings.bytesToHex", lib.srj_bytes_to_hex_sizes, lib.srj_bytes_to_hex)
